@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py -- SparseFusion score-distillation steps/sec on B200 (BASELINE.json metric) + roofline + CPU baseline.
+"""bench.py -- SparseFusion score-distillation steps/sec on H100 (BASELINE.json metric) + roofline + CPU baseline.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" is one iteration of the reference's distillation loop in SDS mode (sparsefusion/distillation.py:174-352, itr > 1000):
@@ -13,8 +13,10 @@ Workload = BASELINE.json configs[2] (the configuration the metric is quoted on):
 With N GPUs every rank runs the step on its own target view (weak scaling over views) and the NGP gradients are all-reduced; `value`
 counts view-steps of all ranks per second.  The max_thres sequence is seeded, identical for every arm and rank.
 
-Printed JSON (rank 0): see the driver contract; `roofline` describes the dominant kernel (the tcgen05 conv/linear GEMM: it streams the
+Printed JSON (rank 0): see the driver contract; `roofline` describes the dominant kernel (the wgmma conv/linear GEMM: it streams the
 UNet's 1.6 GB of fp32 weights once per evaluation), `cpu_baseline` the oracle port of the same step on the host cores.
+--dump-outputs DIR writes what the last timed step returned and left behind (its two losses and the NGP scene parameters) as DIR/<name>.npy,
+float32; the workload is seeded, so runs with the same arguments see the same inputs and two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -50,7 +52,7 @@ def workload_config(world, mean_calls):
     return {'workload': WORKLOAD,
             'parallelism': f'dp{world} over target views, ' + ('no collective' if world == 1 else 'ONE 7.46 MB NGP-gradient all-reduce per step'),
             'unet_evals_per_step_mean': None if mean_calls is None else round(float(mean_calls), 2),
-            'l2': 'inputs larger than L2: each UNet evaluation streams 1.6 GB of fp32 weights (L2 = 126 MB)',
+            'l2': 'inputs larger than L2: each UNet evaluation streams 1.6 GB of fp32 weights (L2 = 50 MB)',
             'lpips': 'LPIPS-VGG perceptual term included in every arm (lambda 0.1, distillation.py:312-314) with seeded random weights -- the lpips '
                      'package and its pretrained weights are un-vendored'}
 
@@ -70,11 +72,11 @@ def peaks():
     try:
         return json.load(open(os.path.join(ROOT, 'MEASURED_PEAKS.json'))), 'measured'
     except Exception:
-        return {'hbm_gbs': 6650.0, 'bf16_tflops': 1590.0, 'bf16_tflops_sustained': 1400.0}, 'fallback'
+        return {'hbm_gbs': 3350.0, 'bf16_tflops': 989.0}, 'fallback'     # H100 SXM data sheet (700 W): HBM3, dense BF16
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md)"""
+    """nvidia-smi clocks / throttle reasons DURING the timed region"""
     Q = ('index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,'
          'clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap')
 
@@ -193,11 +195,14 @@ def run_gpu(args):
         dist.sampler._graph.timing = []
     n_calls = []
     orig_step = step_dev
+    last_losses = []
 
     def step_counting(d, itr, mt):
-        orig_step(d, itr, mt)
+        last_losses[:] = orig_step(d, itr, mt)
         n_calls.append(d.last.get('unet_calls', 0))
     ms = timed(dist, step_counting, K, W)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_losses, dist.ngp)
     clk = clocks.stop() if rank == 0 else None
     launches = ops.launch_count() - l0
     unet_events = dist.sampler._graph.timing if dist.sampler._graph is not None else []
@@ -314,13 +319,13 @@ def run_gpu(args):
                     if k != len(names):
                         break
                     iv = np.diff(stamps) / 1e3
-                    conv_us.append(float(sum(d for nm, d in zip(names[:-1], iv) if nm.startswith('conv_v2'))))
+                    conv_us.append(float(sum(d for nm, d in zip(names[:-1], iv) if nm.startswith('conv<'))))
                     chain_us.append(float(iv.sum()))
             finally:
                 unet.parallel_res_conv = par
             if conv_us:
                 cu = float(np.median(conv_us))
-                n_conv = sum(1 for nm in names if nm.startswith('conv_v2'))
+                n_conv = sum(1 for nm in names if nm.startswith('conv<'))
                 in_graph = {'kernels_per_eval': len(names), 'conv_launches_per_eval': n_conv, 'conv_us_per_eval': round(cu, 1),
                             'eval_us_single_chain': round(float(np.median(chain_us)), 1),
                             'eval_us_first_to_last_kernel': round(float(np.median(all_us)), 1), 'achieved_GBps': round((wb.value / reps) / (cu * 1e-6) / 1e9, 1),
@@ -328,16 +333,8 @@ def run_gpu(args):
                             'note': 'conv_us_per_eval / achieved from a single-chain capture of the same evaluation (per-kernel attribution); '
                                     'eval_us_first_to_last_kernel from the graph the timed region replays (res_conv on a parallel branch)'}
         _lib.call('sfb_trace_end')
-        traffic = None
-        try:    # DRAM bytes per conv launch from the committed ncu --set full capture of this kernel (profiles/, tools/gpu_profile.sh)
-            import csv
-            prof = [f for f in sorted(os.listdir(os.path.join(ROOT, 'profiles'))) if f.endswith('_conv_full_ncu.csv')][-1]
-            rows = list(csv.DictReader(open(os.path.join(ROOT, 'profiles', prof))))
-            traffic = round(sum(float(r['dram_read_MB']) + float(r['dram_write_MB']) for r in rows) * 1e6 / len(rows))
-            traffic_src = f'profiles/{prof}: mean dram__bytes_read.sum + dram__bytes_write.sum over {len(rows)} conv launches of one UNet evaluation'
-        except Exception as e:   # noqa: BLE001
-            traffic_src = f'no ncu capture under profiles/ ({e})'
-        roof = {'kernel': 'conv_gemm_v2_kernel (tcgen05 3xTF32 implicit-GEMM conv/linear, weights streamed from HBM)', 'bound': 'hbm',
+        traffic, traffic_src = None, 'not measured (no DRAM counter capture of this kernel)'
+        roof = {'kernel': 'conv_gemm_kernel (wgmma 3xTF32 implicit-GEMM conv/linear, weights streamed from HBM)', 'bound': 'hbm',
                 'achieved': round(achieved, 1),
                 'peak': pk['hbm_gbs'], 'peak_source': f'{pk_kind} MEASURED_PEAKS.json hbm_gbs (copy bandwidth)', 'unit': 'GB/s',
                 'frac': round(achieved / pk['hbm_gbs'], 4), 'traffic': traffic, 'traffic_source': traffic_src,
@@ -376,7 +373,7 @@ def run_gpu(args):
                'steps': K, 'warmup': W, 'ms_per_step': round(ms / K, 3), 'higher_is_better': True, 'scaling': 'weak', 'vs_baseline': None,
                'dtype': 'f32 (UNet GEMMs: 3xTF32 error-compensated tensor-core passes, fp32 accumulate; NGP: fp32)', 'data': 'synthetic',
                'config': workload_config(world, float(np.mean(n_calls)) if n_calls else None),
-               'engine': {'vae': 'sm_100a engine (tcgen05 3xTF32 convolutions / attention GEMMs, NHWC) -- SURVEY §8f row 1', 'precision_mode': ops.get_precision()},
+               'engine': {'vae': 'sm_90a engine (wgmma 3xTF32 convolutions / attention GEMMs, NHWC) -- SURVEY §8f row 1', 'precision_mode': ops.get_precision()},
                'clocks': clk, 'gpu_launches': int(launches),
                'e2e': None if e2e_val is None else {'value': round(e2e_val, 4), 'unit': 'steps/s', 'h2d_bytes_per_step': int(h2d), 'd2h_bytes_per_step': int(d2h)},
                'roofline': roof, 'cpu_baseline': cpu,
@@ -390,6 +387,19 @@ def run_gpu(args):
         print(json.dumps(out), flush=True)
     if world > 1:
         torch.distributed.destroy_process_group()
+
+
+def dump_outputs(out_dir, losses, ngp):
+    """the last timed step's results as its caller receives them: the two losses Distiller.step returns and the NGP parameters it updated"""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {'loss_photometric': losses[0], 'loss_fusion': losses[1]}
+    arrays.update({'ngp.' + k: v for k, v in ngp.state_dict().items() if v.is_floating_point()})
+    total = 0
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        total += a.nbytes
+        np.save(os.path.join(out_dir, name + '.npy'), a)
+    assert total <= 64 << 20, f'{total} bytes of outputs'
 
 
 class _StagedCache:
@@ -571,8 +581,8 @@ def cpu_baseline(mean_calls):
                       'nothing sampled or scaled. The reference has no CPU path for the NGP render (CUDA-only extensions).'}
 
 
-REF_THREADS = 16     # intra-op threads of the CPU arm: fixed (a start-up probe picked 16 or 32 from run to run); 16 was the fastest count for the 32x32
-                     # feature maps on the 128-thread B200 hosts (tools/cpu_threads_probe.py: 0.26 s per UNet evaluation vs 27.8 s with 128 threads)
+REF_THREADS = 16     # intra-op threads of the CPU arm: fixed (a start-up probe picked 16 or 32 from run to run); more threads than this slow the 32x32
+                     # feature maps down (tools/cpu_threads_probe.py)
 
 
 class CpuWholeStep:
@@ -662,6 +672,8 @@ if __name__ == '__main__':
     ap.add_argument('--c5', action='store_true', help='run the 128x128-latent leg (BASELINE configs[4]); on by default with 8 GPUs')
     ap.add_argument('--no-c5', dest='no_c5', action='store_true', help='skip it with 8 GPUs')
     ap.add_argument('--views', type=int, default=0, help='target views per optimiser step (view-batched step); default: 1 on one GPU, N on N GPUs')
+    ap.add_argument('--dump-outputs', dest='dump_outputs', default=None, metavar='DIR',
+                    help='write the last timed step\'s losses and NGP parameters to DIR/<name>.npy (float32)')
     a = ap.parse_args()
     a.warmup = max(a.warmup, 3) if a.impl == 'ours' else a.warmup
     if a.impl == 'reference':

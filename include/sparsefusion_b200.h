@@ -1,7 +1,7 @@
 /*
  * sparsefusion_b200.h -- C ABI of libsparsefusion_b200.so
  *
- * The drop-in boundary of the B200-native SparseFusion hot path.  Every entry point takes plain
+ * The drop-in boundary of the H100-native SparseFusion hot path.  Every entry point takes plain
  * DEVICE pointers (fp32 / int32 / uint8, contiguous), sizes and a CUDA stream handle
  * (`void* stream` == cudaStream_t; NULL == the legacy default stream); there are no torch types in
  * any signature.  Each function replaces one binding of the reference's pybind operator modules
@@ -53,11 +53,11 @@ int sfb_set_pdl(int on);
 int sfb_trace_begin(unsigned long long* device_buf, unsigned int capacity);
 int sfb_trace_end(void);
 int sfb_trace_names(char* out, int capacity);
-/* phase stamps inside the tcgen05 convolution (CTA 0 of every launch): device_buf[0] = launches seen, device_buf[1 + 8*i + p] = %globaltimer
+/* phase stamps inside the wgmma convolution (CTA 0 of every launch): device_buf[0] = launches seen, device_buf[1 + 8*i + p] = %globaltimer
  * of phase p (0 entry, 1 prologue done, 2 dependency wait returned, 3 first stage converted, 4 last MMA committed, 5 accumulator complete,
  * 6 epilogue done) of launch i < capacity.  NULL unbinds. */
 int sfb_conv_phase_trace(unsigned long long* device_buf, unsigned int capacity);
-/* optional code paths (default all on): bit 0 = the NGP MLP weight gradients run as 3xTF32 tcgen05 GEMMs over the feature-major tapes
+/* optional code paths (default all on): bit 0 = the NGP MLP weight gradients run as 3xTF32 wgmma GEMMs over the feature-major tapes
  * (cleared: the fp32 SIMT outer-product kernel); bit 1 = batch-1 GroupNorm as ONE launch with a software grid barrier between the statistics
  * and the normalisation (cleared: statistics kernel + apply kernel).  Variants agree to fp32 rounding; the switch exists for A/B measurement and tests. */
 int sfb_set_fusion(int mask);
@@ -141,7 +141,7 @@ int sfb_composite_rays(uint32_t n_alive, uint32_t n_step, float T_thresh, int32_
  *    `Unet` module (sparsefusion_b200/imagen_pytorch.py) strings together.
  * ========================================================================================== */
 
-/* nn.Conv2d / nn.Linear as implicit GEMM on tcgen05 tensor cores (kind::tf32, fp32 accumulate), TMA-fed.
+/* nn.Conv2d / nn.Linear as implicit GEMM on wgmma tensor cores (tf32 inputs, fp32 accumulate), TMA-fed.
  * Stands in for Block.project (:652), res_conv (:708), Downsample (:608-610), PixelShuffleUpsample conv
  * (:586), CrossEmbedLayer convs (:1038), ChanFeedForward 1x1 convs (:957,:960), final_conv (:1386) and the
  * token projections of Attention / CrossAttention when there are many tokens.
@@ -175,7 +175,7 @@ int sfb_conv_weight_k(int Cin, int KH, int KW);
 /* per-launch CUDA-event timing of the conv kernel for the roofline line of bench.py (off by default; do not enable under graph capture) */
 int sfb_conv_prof_enable(int on);
 int sfb_conv_prof_collect(double* total_ms, int* launches, double* weight_bytes, double* flops);
-/* 3xTF32 kernel generation: 2 (default) = M-side operand through tensor memory + swap-AB for <= 64 output pixels; 1 = all-smem split */
+/* 3xTF32 kernel generation: 2 (default) = swap-AB for <= 64 output pixels and pre-split weights where given; 1 = neither */
 int sfb_conv_set_variant(int v);
 /* experiment switch: encode activation/weight tensor maps as TFLOAT32 instead of FLOAT32 */
 int sfb_conv_set_tma_tf32(int enable);

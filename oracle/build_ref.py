@@ -4,11 +4,11 @@ TEST INFRASTRUCTURE.  The sources are compiled where they lie under /root/refere
   external/gridencoder/src/{gridencoder.cu,bindings.cpp}   -> oracle/_ref/_ref_gridencoder.so
   raymarching/src/{raymarching.cu,bindings.cpp}            -> oracle/_ref/_ref_raymarching.so
 with the reference's own flags (`-O3 -U__CUDA_NO_HALF_*`, raymarching/backend.py:6-9) except the one-token
-fix `-std=c++14` -> `-std=c++17` that torch >= 2.1 headers need (SURVEY.md §0.10), for sm_100a.
+fix `-std=c++14` -> `-std=c++17` that torch >= 2.1 headers need (SURVEY.md §0.10), for sm_90a.
 
 The resulting pybind modules are the "reference GPU build" of these operators.  They travel to the GPU box
 with the repo snapshot (oracle/_ref/ is git-ignored, not gpurun-ignored) where tests/test_ref_cuda_gpu.py
-checks (a) the C restatement in oracle/ngp_oracle.c and (b) our sm_100a kernels against them.
+checks (a) the C restatement in oracle/ngp_oracle.c and (b) our sm_90a kernels against them.
 """
 from __future__ import annotations
 
@@ -33,7 +33,7 @@ def so_path(name: str) -> str:
 def build(force: bool = False) -> None:
     if not os.path.isdir(REF):
         raise RuntimeError(f'{REF} is not present: oracle/_ref can only be built in the build container')
-    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '10.0a')
+    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '9.0a')
     os.environ.setdefault('MAX_JOBS', '8')
     from torch.utils.cpp_extension import load
     nvcc = ['-O3', '-std=c++17', '-U__CUDA_NO_HALF_OPERATORS__', '-U__CUDA_NO_HALF_CONVERSIONS__', '-U__CUDA_NO_HALF2_OPERATORS__']

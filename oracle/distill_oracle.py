@@ -4,7 +4,7 @@ field), unet_oracle.plms_sample / unet_forward (PLMSSampler + Unet), torch autog
 
 TEST INFRASTRUCTURE ONLY.  Used by tests/test_distillation_gpu.py as the checker of Distiller.step and by bench.py as
 the CPU baseline / `--impl reference` arm (the reference itself has no CPU path for the NGP render -- CUDA-only
-extensions -- and cannot be imported on the GPU box at all; see DESIGN.md).
+extensions -- and cannot be imported on the GPU box at all).
 
 The VAE handed in is oracle/vae_oracle.TorchVAE (torch restatement pinned bit-exact to the reference's Encoder / Decoder by
 tests/golden/vae.npz); the product's AutoencoderKL has no torch / CPU execution path.

@@ -2,7 +2,7 @@
 (external/ldm/models/autoencoder.py:285-333 encode / decode, external/ldm/modules/diffusionmodules/model.py:82-142 ResnetBlock,
 :150-203 AttnBlock, :368-460 Encoder, :462-568 Decoder, external/ldm/modules/distributions/distributions.py:24-62).
 
-TEST INFRASTRUCTURE ONLY (checker for sparsefusion_b200/ldm_autoencoder.py's sm_100a engine, and the VAE of bench.py's CPU /
+TEST INFRASTRUCTURE ONLY (checker for sparsefusion_b200/ldm_autoencoder.py's sm_90a engine, and the VAE of bench.py's CPU /
 eager-GPU baseline arms).  The product never imports this module and has no torch / CPU execution path of its own.
 
 Pinning: oracle/gen_golden.py `vae` loads make_params() into the REFERENCE's own Encoder / Decoder modules (imported from

@@ -1,9 +1,9 @@
-"""Build libsparsefusion_b200.so (the C-ABI library, include/sparsefusion_b200.h) for sm_100a, in tree.
+"""Build libsparsefusion_b200.so (the C-ABI library, include/sparsefusion_b200.h) for sm_90a (H100), in tree.
 
     python -m sparsefusion_b200.build [--force] [--verbose]
 
 Plain nvcc, no torch headers: the library has no torch types in its ABI.  Objects are cached under
-sparsefusion_b200/csrc/_obj and rebuilt by mtime.  nvcc cross-compiles without a GPU.
+sparsefusion_b200/csrc/_obj and rebuilt by mtime or when the flags change.  nvcc cross-compiles without a GPU.
 """
 from __future__ import annotations
 
@@ -18,7 +18,7 @@ CSRC = os.path.join(HERE, 'csrc')
 OBJ = os.path.join(CSRC, '_obj')
 LIB = os.path.join(HERE, 'libsparsefusion_b200.so')
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
-ARCH = ['-gencode', 'arch=compute_100a,code=sm_100a']
+ARCH = ['-gencode', 'arch=compute_90a,code=sm_90a']
 FLAGS = ['-O3', '-std=c++17', '-lineinfo', '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr', '-Xptxas', '-v']
 
 
@@ -48,6 +48,12 @@ def _compile(src: str, force: bool, verbose: bool) -> str:
 
 def build(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(OBJ, exist_ok=True)
+    # objects compiled with other flags (another architecture) are stale whatever their mtime
+    stamp, flags = os.path.join(OBJ, 'flags'), ' '.join([NVCC, *ARCH, *FLAGS])
+    if not os.path.exists(stamp) or open(stamp).read() != flags:
+        force = True
+        with open(stamp, 'w') as f:
+            f.write(flags)
     srcs = sorted(glob.glob(os.path.join(CSRC, '*.cu')))
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(lambda s: _compile(s, force, verbose), srcs))

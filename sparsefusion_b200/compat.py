@@ -1,4 +1,4 @@
-"""Drop-in installation: make the reference's own import statements resolve to the sm_100a modules.
+"""Drop-in installation: make the reference's own import statements resolve to the sm_90a modules.
 
     import sparsefusion_b200.compat as compat
     compat.install()          # before `import demo` / `from utils.load_model import load_models` / `from sparsefusion.distillation import ...`
@@ -54,14 +54,14 @@ _installed: Dict[str, object] = {}
 
 class AutoencoderKL(_AutoencoderKL):
     """external/ldm/models/autoencoder.py:285-310 constructor signature (what ``instantiate_from_config`` calls with the keys of
-    external/ldm/configs/sd-vae.yaml, utils/load_model.py:103-108) over the sm_100a VAE.  ``lossconfig`` / ``monitor`` / ``image_key`` /
+    external/ldm/configs/sd-vae.yaml, utils/load_model.py:103-108) over the sm_90a VAE.  ``lossconfig`` / ``monitor`` / ``image_key`` /
     ``colorize_nlabels`` belong to the training wrapper (pytorch_lightning) and are ignored; ``ckpt_path`` loads like ``init_from_ckpt`` (:312-321)."""
 
     def __init__(self, ddconfig, lossconfig=None, embed_dim=4, ckpt_path=None, ignore_keys=(), image_key='image', colorize_nlabels=None, monitor=None):
         dd = dict(ddconfig)
         assert dd.get('double_z', True), 'the KL autoencoder predicts mean and log-variance (double_z)'
         if tuple(dd.get('attn_resolutions', ())) or float(dd.get('dropout', 0.0)) != 0.0:
-            raise NotImplementedError('sm_100a AutoencoderKL: attn_resolutions / dropout are not part of the SD-v1 KL-f8 configuration (sd-vae.yaml)')
+            raise NotImplementedError('sm_90a AutoencoderKL: attn_resolutions / dropout are not part of the SD-v1 KL-f8 configuration (sd-vae.yaml)')
         super().__init__(ch=int(dd['ch']), ch_mult=tuple(dd['ch_mult']), num_res_blocks=int(dd['num_res_blocks']), in_channels=int(dd['in_channels']),
                          out_ch=int(dd['out_ch']), z_channels=int(dd['z_channels']), embed_dim=int(embed_dim))
         if monitor is not None:

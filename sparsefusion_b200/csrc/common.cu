@@ -88,7 +88,7 @@ int sm_count() {
     int n = cache[dev & 63].load(std::memory_order_relaxed);
     if (n == 0) {
         cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-        if (n <= 0) n = 148;
+        if (n <= 0) n = 132;
         cache[dev & 63].store(n, std::memory_order_relaxed);
     }
     return n;
@@ -116,7 +116,7 @@ int sfb_trace_begin(unsigned long long* device_buf, unsigned int capacity) {
         sfb::g_trace_open = device_buf != nullptr;
     }
     sfb::trace_bind_unet_ops(device_buf, capacity);
-    sfb::trace_bind_conv_v2(device_buf, capacity);
+    sfb::trace_bind_conv(device_buf, capacity);
     SFB_CUDA(cudaGetLastError());
     return SFB_OK;
 }
@@ -126,12 +126,12 @@ int sfb_trace_end(void) {
         sfb::g_trace_open = false;
     }
     sfb::trace_bind_unet_ops(nullptr, 0);
-    sfb::trace_bind_conv_v2(nullptr, 0);
+    sfb::trace_bind_conv(nullptr, 0);
     SFB_CUDA(cudaGetLastError());
     return SFB_OK;
 }
 int sfb_conv_phase_trace(unsigned long long* device_buf, unsigned int capacity) {
-    sfb::phase_bind_conv_v2(device_buf, capacity);
+    sfb::phase_bind_conv(device_buf, capacity);
     SFB_CUDA(cudaGetLastError());
     return SFB_OK;
 }

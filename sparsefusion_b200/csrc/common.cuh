@@ -1,4 +1,4 @@
-// common.cuh -- shared helpers for the sm_100a kernels behind the C-ABI (include/sparsefusion_b200.h)
+// common.cuh -- shared helpers for the sm_90a kernels behind the C-ABI (include/sparsefusion_b200.h)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -31,16 +31,16 @@ int set_precision_override(int m);   // per host thread; -1 = none.  Returns the
 // (b) starts with pdl_sync(): signal that the NEXT kernel may be scheduled, then wait until every kernel before this one has completed
 // and flushed its memory.  All global reads and writes of a kernel come after that wait, so ordering is unchanged.
 bool pdl_enabled();
-// Every PDL-launched kernel asks for the maximum shared-memory carve-out, whether it needs it or not: the tcgen05 convolutions use ~200 KB of
+// Every PDL-launched kernel asks for the maximum shared-memory carve-out, whether it needs it or not: the wgmma convolutions use ~200 KB of
 // smem, and a dependent kernel can only become resident next to the draining CTAs of its predecessor (the point of PDL) when both want the
 // same L1/shared split of the SM.
 void prefer_smem(const void* kernel);
 size_t pad_smem(const void* kernel, size_t smem);   // experiment (sfb_set_pdl bit 2): every PDL kernel requests a conv-sized dynamic smem block
 void trace_name(const char* kernel);   // host side of the tracer: kernel names in launch order while a trace is open
 void trace_bind_unet_ops(unsigned long long* buf, unsigned int cap);
-void trace_bind_conv_v2(unsigned long long* buf, unsigned int cap);
-void phase_bind_conv_v2(unsigned long long* buf, unsigned int cap);
-// optional paths (sfb_set_fusion): bit 0 = NGP MLP weight gradients as tcgen05 GEMMs (off: the SIMT outer-product kernel)
+void trace_bind_conv(unsigned long long* buf, unsigned int cap);
+void phase_bind_conv(unsigned long long* buf, unsigned int cap);
+// optional paths (sfb_set_fusion): bit 0 = NGP MLP weight gradients as wgmma GEMMs (off: the SIMT outer-product kernel)
 int fusion_mask();
 static inline bool wgrad_tc_enabled() { return (fusion_mask() & 1) != 0; }
 static inline bool field_v2_enabled() { return (fusion_mask() & 16) != 0; }    // tiled NGP field kernels (128-point GEMM tiles in shared memory, no tape)

@@ -1,9 +1,9 @@
-// eft_ops.cu -- the non-GEMM operators of the Epipolar Feature Transformer (sparsefusion/eft.py, SURVEY.md §8f row 4), NHWC fp32, sm_100a.
+// eft_ops.cu -- the non-GEMM operators of the Epipolar Feature Transformer (sparsefusion/eft.py, SURVEY.md §8f row 4), NHWC fp32, sm_90a.
 //
 // The EFT builds the per-view conditioning cache once per scene (sparsefusion/distillation.py:92-127): a ResNet-18 pyramid over the input views
 // (eft.py:172-204), bilinear look-ups of that pyramid at the projections of every ray sample (F.grid_sample, eft.py:248-275), and three small
 // transformer encoders over (input views) / (depth samples) / (input views) (eft.py:396-440).  Convolutions and every nn.Linear run on the
-// tcgen05 implicit-GEMM engine (conv_tcgen05*.cu); this file holds what is left: 3x3/2 max-pooling, bilinear resize (align_corners), the
+// wgmma implicit-GEMM engine (conv_wgmma.cu); this file holds what is left: 3x3/2 max-pooling, bilinear resize (align_corners), the
 // grid-sample gather, the single-head attention core over short sequences, and the in-place activations.  All latency / L2-gather bound.
 #include "common.cuh"
 #include "../../include/sparsefusion_b200.h"

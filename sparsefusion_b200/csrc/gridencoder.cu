@@ -1,4 +1,4 @@
-// gridencoder.cu -- multi-resolution tiled/hash grid encoder operators for sm_100a.
+// gridencoder.cu -- multi-resolution tiled/hash grid encoder operators for sm_90a.
 //
 // Drop-in for the reference's `_gridencoder` pybind module (external/gridencoder/src/bindings.cpp:5-8):
 // same argument order and layouts ([L,B,C] level-major outputs, [B,L,D,C] dy_dx, pre-zeroed gradient
@@ -7,7 +7,7 @@
 // tiled-index quirk that drops trailing coordinates once the running stride exceeds the level's row
 // count -- so that embeddings trained by either implementation are interchangeable.
 //
-// B200 notes: the whole live table is 7.1 MB and lives in the 126 MB L2, so these kernels are L2-gather
+// H100 notes: the whole live table is 7.1 MB and lives in the 50 MB L2, so these kernels are L2-gather
 // bound; what matters is (a) one 8-byte gather per corner for C == 2 (float2), (b) coalesced [L,B,C]
 // stores, (c) for the backward, one vector reduction (red.global.add.v2.f32) per corner instead of C
 // scalar atomics.  The fused field kernels in ngp_field.cu are the hot path; these operators exist for

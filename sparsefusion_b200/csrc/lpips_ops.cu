@@ -1,8 +1,8 @@
 // lpips_ops.cu -- SURVEY.md section 8f row 3: the LPIPS-VGG perceptual term of the fusion loss (sparsefusion/distillation.py:312-314 through
 // external/external_utils.py:11-49 -> lpips.LPIPS(net='vgg'), Zhang et al. CVPR 2018), forward AND the gradient w.r.t. the rendered image.
 //
-// The thirteen 3x3 convolutions (and their data-gradient convolutions, same kernel with transposed / flipped weights) run on the tcgen05
-// implicit-GEMM engine (conv_tcgen05*.cu); this file holds what surrounds them, all NHWC fp32:
+// The thirteen 3x3 convolutions (and their data-gradient convolutions, same kernel with transposed / flipped weights) run on the wgmma
+// implicit-GEMM engine (conv_wgmma.cu); this file holds what surrounds them, all NHWC fp32:
 //   lpips_prep        (2 img - 1 - shift) / scale of both images -> [2,H,W,4] (4th channel zero: TMA wants 16-byte pixels)
 //   relu              in place
 //   maxpool2x2        forward; backward routes the gradient to the first maximum of each window (torch semantics) and applies the ReLU mask of

@@ -1,4 +1,4 @@
-// ngp_field.cu -- the Instant-NGP field query of SparseFusion's NeRFNetwork, fused, for sm_100a:
+// ngp_field.cu -- the Instant-NGP field query of SparseFusion's NeRFNetwork, fused, for sm_90a:
 //     xyz -> tiled-grid encode (16 levels x 2) -> MLP 32-64-64-4 (ReLU) -> sigma = exp(h0 + blob(x)), albedo = sigmoid(h1:4)
 // (external/nerf/network_grid.py:69-88 common_forward; external/gridencoder/grid.py:138-154; ngp_activation.py:10-21).
 // The reference runs this as ~12 eager launches per call (kernel_grid + permute + 3 cuBLAS GEMMs + elementwise) and
@@ -1039,7 +1039,7 @@ int sfb_ngp_field_backward(const float* xyz, const float* rays_o, const float* r
                                                               grad_embeddings, H0, H1, H2, D1, D2, D3);
     if (int rc = check_launch("ngp_field_backward(data)")) return rc;
     if (wgrad_tc_enabled()) {
-        // dW = D . H^T with the point index as the GEMM's K dimension: the feature-major tapes are exactly the K-major operands the tcgen05
+        // dW = D . H^T with the point index as the GEMM's K dimension: the feature-major tapes are exactly the K-major operands the wgmma
         // implicit-GEMM kernel streams (rows of D = "pixels", rows of H = "output channels", 1x1 tap), 3xTF32, split-K over the 2.1 M points
         // with fp32 reductions into the gradient buffers (accumulate = 1).  Bias gradients are row sums of D.
         const int old = set_precision_override(1);

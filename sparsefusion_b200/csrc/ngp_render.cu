@@ -1,4 +1,4 @@
-// ngp_render.cu -- the per-ray stages of NeRFRenderer.run (external/nerf/renderer_df.py:310-468), fused for sm_100a.
+// ngp_render.cu -- the per-ray stages of NeRFRenderer.run (external/nerf/renderer_df.py:310-468), fused for sm_90a.
 //
 // The reference expresses these as ~120 eager PyTorch launches per render (linspace / rand / cumprod / searchsorted /
 // gather / sort / sum ...), all on [N,64] or [N,128] tensors.  Here one WARP owns one ray and keeps the ray's samples in

@@ -1,5 +1,5 @@
 // raymarching.cu -- ray/aabb, morton, bit-packing, occupancy-grid marching and compositing operators
-// for sm_100a.  Drop-in for the reference's `_raymarching` pybind module
+// for sm_90a.  Drop-in for the reference's `_raymarching` pybind module
 // (raymarching/src/bindings.cpp:5-18): same argument order, layouts and in-place conventions, fp32.
 //
 // Integer contract kept bit-identical to raymarching/src/raymarching.cu: morton codes (:56-81), mip
@@ -8,7 +8,7 @@
 // exactly like the reference (:405-406), so point layout is not deterministic -- consumers go through
 // the `rays` table.
 //
-// B200 notes: one thread per ray is kept for the marchers (divergent DDA loops); they are bound by the
+// H100 notes: one thread per ray is kept for the marchers (divergent DDA loops); they are bound by the
 // 786 KB occupancy bitfield which stays in L1/L2.  The compositing kernels read three streams
 // (sigma 4 B, rgb 12 B, delta 8 B per point) -- HBM-bound, so each thread walks its ray's contiguous
 // point range with independent loads in flight.

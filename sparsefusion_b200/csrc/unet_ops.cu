@@ -1,4 +1,4 @@
-// unet_ops.cu -- the non-GEMM operators of the VLDM UNet forward, NHWC fp32, for sm_100a.
+// unet_ops.cu -- the non-GEMM operators of the VLDM UNet forward, NHWC fp32, for sm_90a.
 //
 // They replace the eager PyTorch elementwise / normalisation / tiny-attention launches of the
 // reference's Unet (external/imagen_pytorch.py): GroupNorm+FiLM+SiLU of `Block` (:654-662), gain-only
@@ -7,10 +7,10 @@
 // (:936-941), PixelShuffle(2)+SiLU (:588-592), skip concatenation (:1639), the learned sinusoidal time
 // embedding (:634-639) and small-M Linear layers (time MLPs, token projections), which are weight
 // streaming GEMVs and stay in full fp32.
-// Tensors that feed a tcgen05 GEMM are rounded to TF32 (cvt.rna) when they are written here, so the
+// Tensors that feed a wgmma GEMM are rounded to TF32 (cvt.rna) when they are written here, so the
 // tensor core's operand truncation never biases the result.
 #include "common.cuh"
-#include "tcgen05.cuh"
+#include "wgmma.cuh"
 #include <cooperative_groups.h>
 #include "../../include/sparsefusion_b200.h"
 

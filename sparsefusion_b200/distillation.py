@@ -8,8 +8,8 @@ and the per-view EFT features / images arrive cached (:95-125).  Loss formulas, 
 RNG draws follow the reference line by line (citations inline).  ``INTEGRATION.md`` shows how the reference's
 ``distillation_loop`` calls this.
 
-What runs where: both NGP renders (fused sm_100a kernels, analytic backward), the PLMS sampler's UNet evaluations
-(tcgen05 engine, one CUDA graph replay per evaluation), the SD VAE encode / decode (``ldm_autoencoder.py``, same engine), the
+What runs where: both NGP renders (fused sm_90a kernels, analytic backward), the PLMS sampler's UNet evaluations
+(wgmma engine, one CUDA graph replay per evaluation), the SD VAE encode / decode (``ldm_autoencoder.py``, same engine), the
 image-space losses with their gradients (``image_glue.py``), the LPIPS-VGG term when a ``percep`` module is given (``lpips_vgg.py``;
 :312-314), fused Adam.
 

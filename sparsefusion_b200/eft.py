@@ -5,14 +5,14 @@ for every cached view (sparsefusion/distillation.py:92-127; SURVEY.md §8f row 4
 Same constructor keywords, ``encode(input_cameras, input_images)``, ``forward(ray_bundle, **kwargs)``, ``batched_forward(ray_bundle, n_batches,
 **kwargs)`` and the same state_dict keys (``encoder_model.*`` = torchvision's resnet18, ``t1|t2|t3.pre.0``, ``t*.encoder.layers.N.{self_attn.in_proj_*,
 self_attn.out_proj, linear1, linear2, norm1, norm2}``, ``t2_attn``, ``t3_attn``, ``color_layer.0``), so utils/load_model.py:34-41 loads its
-checkpoint unchanged.  The torch modules registered here are PARAMETER CONTAINERS; the arithmetic runs on the sm_100a engine:
+checkpoint unchanged.  The torch modules registered here are PARAMETER CONTAINERS; the arithmetic runs on the sm_90a engine:
 
-* ResNet-18 pyramid (eft.py:172-204): every convolution on the tcgen05 implicit-GEMM kernel with the (eval-mode) BatchNorm folded into the
+* ResNet-18 pyramid (eft.py:172-204): every convolution on the wgmma implicit-GEMM kernel with the (eval-mode) BatchNorm folded into the
   packed weights, ReLU / residual adds in its epilogue or one elementwise pass, 3x3/2 max-pool, bilinear (align_corners) resize of the four
   levels into ONE 512-channel NHWC tensor;
 * epipolar look-up (eft.py:230-275): ``grid_sample`` of that tensor and of the input images at the NDC projections of all ray samples, one
   warp per point, written straight into the (padded) token rows of transformer T1;
-* T1 / T2 / T3 (eft.py:18-50, :396-440): nn.TransformerEncoder(4 layers, d 256, 1 head, ff 256, post-norm, ReLU) as tcgen05 linears (3xTF32) +
+* T1 / T2 / T3 (eft.py:18-50, :396-440): nn.TransformerEncoder(4 layers, d 256, 1 head, ff 256, post-norm, ReLU) as wgmma linears (3xTF32) +
   a one-warp-per-query attention core over the short sequences (2-6 views or 20 depth samples) + the fused residual LayerNorm kernel.
 
 Camera maths (pytorch3d's PerspectiveCameras in NDC: x_view = x_world R + T, x_ndc = f x/z + p; centre = -T R^T) is used through the camera
@@ -88,7 +88,7 @@ class TransformerEncoder(nn.Module):
         self.encoder = nn.TransformerEncoder(nn.TransformerEncoderLayer(n_hidden, 1, n_hidden, 0.1), n_layer, enable_nested_tensor=False)
 
     def forward(self, *a, **k):
-        raise RuntimeError('TransformerEncoder is a parameter container of sparsefusion_b200.EpipolarFeatureTransformer (sm_100a engine; no torch path)')
+        raise RuntimeError('TransformerEncoder is a parameter container of sparsefusion_b200.EpipolarFeatureTransformer (sm_90a engine; no torch path)')
 
 
 class EpipolarFeatureTransformer(nn.Module):

@@ -4,7 +4,7 @@
 identical: 477 tensors for the SparseFusion config, utils/load_model.py:58-69), ``forward`` /
 ``forward_with_cond_scale`` / ``cast_model_parameters`` signatures and NCHW tensors at the boundary, so
 ``sparsefusion/vldm.py`` (DDPM), ``external/plms.py`` and ``utils/load_model.py`` use it unchanged.  The forward
-itself never touches torch.nn: it is a sequence of sm_100a kernels from libsparsefusion_b200.so (tcgen05
+itself never touches torch.nn: it is a sequence of sm_90a kernels from libsparsefusion_b200.so (wgmma
 implicit-GEMM convolutions + fused norm/attention kernels, NHWC) launched on the current stream, and can be
 captured into a CUDA graph (``UnetGraph``).  It is inference-only: SparseFusion's distillation loop runs the UNet
 under no_grad (sparsefusion/distillation.py:302-304).
@@ -418,7 +418,7 @@ class Unet(nn.Module):
 
     def _linear_rows(self, name, x, bias=True, round_out=False):
         """token projection [.., K] -> [.., O]: fp32 GEMV for a handful of rows, tensor cores (swap-AB tile: the rows are the N side) from 16 rows up --
-        in the replayed graph the 8-row GEMV tile costs 13.8 us per projection of the 4x4 stage's 16 tokens, the tcgen05 path ~5 us"""
+        in the replayed graph the 8-row GEMV tile costs 13.8 us per projection of the 4x4 stage's 16 tokens, the wgmma path ~5 us"""
         pl = self._plan
         w = pl['P'][name + '.weight']
         b = pl['P'].get(name + '.bias') if bias else None
@@ -468,7 +468,7 @@ class Unet(nn.Module):
             if join is not None:
                 torch.cuda.current_stream().wait_stream(join)
             # (GlobalContext + gate + residual as ONE thread-block-cluster kernel was built and measured: 21 us per block against 16.9 us for these four
-            #  launches -- five dependent global / DSMEM round trips do not shrink by sharing a launch -- and taken out again; DESIGN.md §3.2)
+            #  launches -- five dependent global / DSMEM round trips do not shrink by sharing a launch -- and taken out again)
             out = ops.gate_mlp_residual(h2, hid, w2.reshape(w2.shape[0], -1), P[f'{pfx}.gca.net.2.bias'], res)   # gate GEMV + sigmoid + h*gate + res
         else:
             if join is not None:

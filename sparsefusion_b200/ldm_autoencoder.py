@@ -6,8 +6,8 @@ SURVEY.md §8f "next" row #1.  Same module tree and state_dict keys as the refer
 ``quant_conv``, ``post_quant_conv``), without the pytorch_lightning / taming base classes the reference drags in.
 
 ONE execution path behind ``encode`` / ``decode`` (both inference-only in the loop: ``vae.encode(...).mode()`` at
-sparsefusion/distillation.py:299 and ``vae.decode(...)`` at :309 run under no_grad): the sm_100a engine (``_Sm100Engine`` below) -- NHWC
-activations, every convolution / 1x1 projection / attention matmul on the tcgen05 3xTF32 implicit-GEMM kernel (``ops.conv2d_nhwc``),
+sparsefusion/distillation.py:299 and ``vae.decode(...)`` at :309 run under no_grad): the sm_90a engine (``_Sm90Engine`` below) -- NHWC
+activations, every convolution / 1x1 projection / attention matmul on the wgmma 3xTF32 implicit-GEMM kernel (``ops.conv2d_nhwc``),
 GroupNorm(32)+swish fused in one pass over the data, nearest upsampling and the row softmax as small kernels.  No cuDNN, no torch matmul,
 no CPU fallback: the module classes below are PARAMETER CONTAINERS with the reference's names and shapes (checkpoints load unchanged);
 calling them, or calling encode / decode with non-CUDA tensors, raises.  The plain-torch restatement that checks this engine lives in
@@ -24,10 +24,10 @@ def _norm(c):
 
 
 class _Container(nn.Module):
-    """parameter container: the arithmetic of these blocks runs in _Sm100Engine, never through torch.nn"""
+    """parameter container: the arithmetic of these blocks runs in _Sm90Engine, never through torch.nn"""
 
     def forward(self, *a, **k):
-        raise RuntimeError(f'{type(self).__name__} is a parameter container of sparsefusion_b200.AutoencoderKL: the VAE runs on the sm_100a engine '
+        raise RuntimeError(f'{type(self).__name__} is a parameter container of sparsefusion_b200.AutoencoderKL: the VAE runs on the sm_90a engine '
                            '(AutoencoderKL.encode / decode with CUDA tensors); there is no torch / CPU execution path')
 
 
@@ -143,8 +143,8 @@ class DiagonalGaussianDistribution:
         return self.mean + self.std * torch.randn_like(self.mean)
 
 
-class _Sm100Engine:
-    """Encoder / Decoder forward on the sm_100a operators (NHWC, 3xTF32 tensor cores).  Weights are packed once (``prepare``)."""
+class _Sm90Engine:
+    """Encoder / Decoder forward on the sm_90a operators (NHWC, 3xTF32 tensor cores).  Weights are packed once (``prepare``)."""
 
     GROUPS, EPS = 32, 1e-6
 
@@ -154,7 +154,7 @@ class _Sm100Engine:
         self.vae = vae
         P = {n: p.detach() for n, p in vae.named_parameters()}
         if next(iter(P.values())).device.type != 'cuda':
-            raise RuntimeError('the sm_100a VAE engine needs CUDA parameters')
+            raise RuntimeError('the sm_90a VAE engine needs CUDA parameters')
         self.P, self.W, self.B, self.S = P, {}, {}, {}
         for n, p in P.items():
             if n.endswith('.weight') and p.dim() == 4:
@@ -188,7 +188,7 @@ class _Sm100Engine:
         nb, hh, ww, c = x.shape
         n = hh * ww
         if n % 32 or c % 32:
-            raise NotImplementedError('sm_100a VAE attention needs h*w and channels to be multiples of 32')
+            raise NotImplementedError('sm_90a VAE attention needs h*w and channels to be multiples of 32')
         hn = self.gn(pfx + '.norm', x, False)
         out = torch.empty_like(x)
         wv = self.P[pfx + '.v.weight'].reshape(c, c)
@@ -255,15 +255,15 @@ class AutoencoderKL(nn.Module):
         self._sm100 = None
 
     def prepare(self):
-        """(re)pack the weights for the sm_100a engine; call again after loading a checkpoint or switching ops.set_precision"""
-        self._sm100 = _Sm100Engine(self)
+        """(re)pack the weights for the sm_90a engine; call again after loading a checkpoint or switching ops.set_precision"""
+        self._sm100 = _Sm90Engine(self)
         return self
 
     def _engine_for(self, t):
         if not t.is_cuda:
-            raise RuntimeError('sparsefusion_b200.AutoencoderKL runs on CUDA tensors only (sm_100a engine; there is no CPU fallback)')
+            raise RuntimeError('sparsefusion_b200.AutoencoderKL runs on CUDA tensors only (sm_90a engine; there is no CPU fallback)')
         if torch.is_grad_enabled() and (t.requires_grad or any(p.requires_grad for p in self.parameters())):
-            raise RuntimeError('the sm_100a VAE engine is inference-only (the distillation loop calls the VAE under no_grad): wrap the call in '
+            raise RuntimeError('the sm_90a VAE engine is inference-only (the distillation loop calls the VAE under no_grad): wrap the call in '
                                'torch.no_grad()')
         if self._sm100 is None:
             self.prepare()

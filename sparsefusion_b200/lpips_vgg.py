@@ -10,7 +10,7 @@ no_grad, distillation.py:302-309).
 weights load unchanged; this repository cannot ship them (no network), so a fresh module is randomly initialised and says so.
 
 Engine (CUDA only, C ABI section 7): both images go through the VGG16 trunk as ONE batch of two NHWC tensors; the 13 convolutions and, for the
-gradient, their 13 data-gradient convolutions (same kernel, weights transposed and flipped) run on the tcgen05 3xTF32 implicit-GEMM engine with
+gradient, their 13 data-gradient convolutions (same kernel, weights transposed and flipped) run on the wgmma 3xTF32 implicit-GEMM engine with
 pre-split weights; ReLU / 2x2 max-pool (forward, and backward fused with the ReLU mask) / the per-tap LPIPS head (value and gradient in one
 launch) / input scaling are small NHWC kernels.  Value and gradient are produced together; autograd only sees one custom Function.
 """

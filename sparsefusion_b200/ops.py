@@ -90,7 +90,7 @@ def _rows_meta(t: torch.Tensor) -> Tuple[int, int, int]:
 
 # --------------------------------------------------------------------------------------------- conv / linear on tensor cores
 # --------------------------------------------------------------------------------------------- split-K output arena
-# The weight-streaming convolutions split K over up to 148 CTAs and meet in fp32 red.global.add, so their destination must start from
+# The weight-streaming convolutions split K over up to one CTA per SM and meet in fp32 red.global.add, so their destination must start from
 # zero.  One cudaMemset node per convolution costs ~2.3 us inside the replayed UNet graph (and breaks the programmatic-dependent-launch
 # edge in front of the convolution); with an arena all conv outputs of one UNet evaluation are carved out of ONE buffer that is
 # zero-filled once at the start of the evaluation, and the convolutions run in "accumulate" mode.

@@ -6,7 +6,7 @@ return values ``(pred_x0, x_noisy, noise, alpha_cumprod)``.  ``n_steps = min(int
 steps, ``n_steps + 1`` UNet evaluations (plms.py:87,136-142), Adams-Bashforth 2/3/4 on the eps history (:144-152),
 clamp of x0 to +-clip_value (:205), stochastic posterior step (:208-212).
 
-B200 notes: each eps evaluation replays one CUDA graph of the UNet (``UnetGraph``); the schedule scalars (alpha, sigma, c,
+H100 notes: each eps evaluation replays one CUDA graph of the UNet (``UnetGraph``); the schedule scalars (alpha, sigma, c,
 posterior variance) are computed on the host from t / t_next and the whole latent update of a step -- Adams-Bashforth
 combination, x0 prediction + clamp, posterior mean, noise injection: ~30 eager launches in the reference -- is ONE fused
 kernel (``sfb_plms_update``).  Every ``torch.randn_like`` of the reference is routed through ``self.noise_fn`` (default

@@ -11,7 +11,7 @@ Same class / method names and keyword arguments (``render``, ``render_batched``,
 launches and evaluates the field three times (coarse, fine, colour); here it is seven kernels and every point is
 evaluated once per role (coarse density for the sampling pdf, then sigma+rgb at the 128 sorted samples), with an
 analytic backward -- gradients equal the reference's because its fine/colour passes see the same points and
-parameters (DESIGN.md spells out the argument).
+parameters.
 """
 from __future__ import annotations
 

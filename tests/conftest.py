@@ -1,4 +1,4 @@
-"""pytest configuration: `gpu` marker for tests that need a B200 (everything else runs on CPU)."""
+"""pytest configuration: `gpu` marker for tests that need a H100 (everything else runs on CPU)."""
 import os
 import sys
 
@@ -11,7 +11,7 @@ GOLDEN = os.path.join(ROOT, 'tests', 'golden')
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box with `-m gpu`)')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the H100 box with `-m gpu`)')
 
 
 def pytest_collection_modifyitems(config, items):

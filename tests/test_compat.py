@@ -78,15 +78,21 @@ def test_aliases_resolve_and_construct_with_load_model_kwargs():
     assert 'external.imagen_pytorch' not in sys.modules and 'sparsefusion.vldm' not in sys.modules
 
 
-@pytest.mark.skipif(not os.path.isdir('/root/reference'), reason='needs the reference tree (build container only)')
-def test_aliases_shadow_the_reference_tree_when_it_is_on_the_path():
-    """with /root/reference first on sys.path (how demo.py runs), install() must win over the reference's own modules of the same names"""
-    code = ("import sys; sys.dont_write_bytecode = True; sys.path.insert(0, '/root/reference'); sys.path.insert(0, %r)\n"
+def test_aliases_shadow_the_reference_tree_when_it_is_on_the_path(tmp_path):
+    """with the reference's tree first on sys.path (how demo.py runs), install() must win over the reference's own modules of the same names.
+    The tree here is a stand-in with the reference's package layout whose modules define the same names."""
+    ref = tmp_path / 'reference'
+    for pkg, mods in {'external': {'imagen_pytorch': 'Unet', 'plms': 'PLMSSampler'}, 'sparsefusion': {'vldm': 'DDPM', 'distillation': 'distillation_loop'}}.items():
+        (ref / pkg).mkdir(parents=True)
+        (ref / pkg / '__init__.py').write_text('')
+        for mod, name in mods.items():
+            (ref / pkg / f'{mod}.py').write_text(f'{name} = None\n')
+    code = ("import sys; sys.dont_write_bytecode = True; sys.path.insert(0, %r); sys.path.insert(0, %r)\n"
             "import sparsefusion_b200.compat as c; c.install()\n"
             "from external.imagen_pytorch import Unet\nfrom external.plms import PLMSSampler\nfrom sparsefusion.vldm import DDPM\n"
             "from sparsefusion.distillation import distillation_loop\nimport external\n"
             "assert Unet.__module__ == 'sparsefusion_b200.imagen_pytorch' and PLMSSampler.__module__ == 'sparsefusion_b200.plms'\n"
             "assert DDPM.__module__ == 'sparsefusion_b200.vldm' and distillation_loop.__module__ == 'sparsefusion_b200.distillation'\n"
-            "assert external.__path__ and 'reference' in list(external.__path__)[0]\nprint('ok')\n") % ROOT
-    out = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=300, cwd='/tmp')
+            "assert external.__path__ and 'reference' in list(external.__path__)[0]\nprint('ok')\n") % (str(ref), ROOT)
+    out = subprocess.run([sys.executable, '-c', code], capture_output=True, text=True, timeout=300, cwd=str(tmp_path))
     assert out.returncode == 0 and out.stdout.strip().endswith('ok'), out.stderr[-2000:]

@@ -1,4 +1,4 @@
-"""tcgen05 implicit-GEMM convolution (sfb_conv2d_nhwc_tf32) against a plain PyTorch reference (fp64 accumulate).
+"""wgmma implicit-GEMM convolution (sfb_conv2d_nhwc_tf32) against a plain PyTorch reference (fp64 accumulate).
 
 Tolerances, all written here:
   * operands pre-rounded to TF32 on both sides -> only the fp32 accumulation order differs: rel L2 <= 2e-6 (both modes);

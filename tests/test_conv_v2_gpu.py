@@ -1,5 +1,5 @@
-"""Second-generation 3xTF32 conv kernel (M-side operand through tensor memory, swap-AB for <= 64 output pixels) against fp64
-references and against the first-generation kernel.  Tolerance: fp32-class, rel L2 <= 1e-5 (the accumulation chain per CTA is capped at 96 k-steps; longer chains drift, see conv_tcgen05.cu)."""
+"""Second-generation 3xTF32 conv kernel (M-side operand split in registers, swap-AB for <= 64 output pixels) against fp64
+references and against the first-generation kernel.  Tolerance: fp32-class, rel L2 <= 1e-5 (the accumulation chain per CTA is capped at 96 k-steps; longer chains drift, see conv_wgmma.cu)."""
 import pytest
 import torch
 import torch.nn.functional as F
@@ -60,7 +60,7 @@ def test_v2_matches_reference_and_v1(case):
 
 def test_tensor_core_reads_tf32_by_truncation():
     """Experiment recorded as a test: feeding the un-masked fp32 word as the 'hi' operand (variant 3) must give bit-identical
-    results to the explicitly masked operand (variant 2) if -- and only if -- kind::tf32 ignores the 13 low mantissa bits."""
+    results to the explicitly masked operand (variant 2) if -- and only if -- the tensor core's tf32 read ignores the 13 low mantissa bits."""
     from sparsefusion_b200 import _lib as lib, ops
     ops.set_precision('tf32x3')
     g = torch.Generator(device='cuda').manual_seed(5)

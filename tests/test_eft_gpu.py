@@ -1,4 +1,4 @@
-"""Epipolar Feature Transformer on the sm_100a engine (SURVEY §8f row 4) against tests/golden/eft.npz -- outputs of the REFERENCE's own
+"""Epipolar Feature Transformer on the sm_90a engine (SURVEY §8f row 4) against tests/golden/eft.npz -- outputs of the REFERENCE's own
 EpipolarFeatureTransformer (sparsefusion/eft.py) on the same deterministic weights and inputs -- and its new operators against torch.
 Bar: 1e-3 relative L2 (BASELINE.json north_star tolerance for floating-point outputs)."""
 import numpy as np

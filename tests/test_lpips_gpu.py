@@ -1,4 +1,4 @@
-"""LPIPS-VGG perceptual term (SURVEY §8f row 3) on the sm_100a engine against the torch restatement of the published algorithm
+"""LPIPS-VGG perceptual term (SURVEY §8f row 3) on the sm_90a engine against the torch restatement of the published algorithm
 (oracle/lpips_oracle.py, fp64, autograd) with identical seeded weights.  Parity with the pretrained lpips package is unpinned (its
 weights cannot be fetched); what is pinned: value within 1e-3 relative, gradient w.r.t. the rendered image within 1e-3 relative L2."""
 import pytest

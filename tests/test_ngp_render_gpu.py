@@ -42,7 +42,7 @@ def test_state_dict_keys_match_reference_checkpoint_layout():
 @pytest.fixture(params=[0x7fffffff, 0x7fffffff & ~16, 0], ids=['field-v2-tiled', 'field-v1-wgrad-tcgen05', 'field-v1-wgrad-simt'])
 def wgrad_path(request):
     """the three implementations of the field kernels: v2 = 128-point GEMM tiles in shared memory with in-register weight gradients (default,
-    sfb_set_fusion bit 4); v1 = one point per thread + activation tapes, with the weight gradients as tcgen05 GEMMs (bit 0) or a SIMT outer product"""
+    sfb_set_fusion bit 4); v1 = one point per thread + activation tapes, with the weight gradients as wgmma GEMMs (bit 0) or a SIMT outer product"""
     from sparsefusion_b200 import _lib as lib
     lib.call('sfb_set_fusion', request.param)
     yield request.param

@@ -1,146 +1,90 @@
-"""Cross-validation against the REFERENCE's own CUDA operators (oracle/_ref/*.so, built by oracle/build_ref.py
-from /root/reference's sources with the c++17 one-token patch): (a) our sm_100a kernels, (b) the C restatement.
+"""Cross-validation against the REFERENCE's own CUDA operators: tests/golden/ref_cuda.npz holds their outputs on seeded inputs
+(oracle/ref_cuda_golden.py, run on a GPU against the reference's sources compiled by oracle/build_ref.py).  Checked here against them:
+(a) our sm_90a kernels, (b) the C restatement.
 
 This is what pins the NGP half of the oracle to the reference: the reference has no tests or golden vectors
-for this path, and its operators are CUDA-only, so they can only run here, on the GPU box.
+for this path, and its operators are CUDA-only.
 """
 import numpy as np
 import pytest
 import torch
 
+from oracle import ref_cuda_golden as rg
+
 pytestmark = pytest.mark.gpu
 
 
-def _ref(name):
-    import os
-    from oracle import build_ref
-    if not os.path.exists(build_ref.so_path(name)):
-        pytest.skip(f'oracle/_ref/{name}.so not built (needs /root/reference at build time)')
-    return build_ref.load_module(name)
+@pytest.fixture(scope='module')
+def gold(golden_dir):
+    return np.load(f'{golden_dir}/ref_cuda.npz')
 
 
-def _grid_problem(B=1 << 18, seed=0):
-    from oracle import ngp_oracle as no
-    geo = no.live_geometry()
-    rng = np.random.default_rng(seed)
-    x = np.concatenate([rng.random((B, 3), dtype=np.float32), no.golden_grid_inputs()])
-    emb = no.make_field_params(seed=1)['encoder.embeddings']
-    return geo, x, emb
-
-
-def test_grid_forward_bit_identical_to_reference_cuda():
-    ref = _ref('_ref_gridencoder')
+def test_grid_forward_bit_identical_to_reference_cuda(gold):
     from sparsefusion_b200 import _gridencoder as ours
-    geo, x, emb = _grid_problem()
+    geo, x, emb = rg.grid_problem(1 << 18)
     B, L, C, D = x.shape[0], geo['L'], geo['C'], 3
     xt, et, off = torch.from_numpy(x).cuda(), emb.cuda(), torch.from_numpy(geo['offsets']).cuda()
-    o_ref, o_our = torch.empty(L, B, C, device='cuda'), torch.empty(L, B, C, device='cuda')
-    d_ref, d_our = torch.empty(B, L * D * C, device='cuda'), torch.empty(B, L * D * C, device='cuda')
-    ref.grid_encode_forward(xt, et, off, o_ref, B, D, C, L, geo['S'], geo['H'], d_ref, 1, False)
+    o_our, d_our = torch.empty(L, B, C, device='cuda'), torch.empty(B, L * D * C, device='cuda')
     ours.grid_encode_forward(xt, et, off, o_our, B, D, C, L, geo['S'], geo['H'], d_our, 1, False)
     torch.cuda.synchronize()
     # identical indices AND identical interpolation arithmetic -> identical bits
-    assert torch.equal(o_ref, o_our), f'{(o_ref != o_our).sum().item()} of {o_ref.numel()} outputs differ, max {(o_ref - o_our).abs().max().item():.3e}'
-    assert torch.allclose(d_ref, d_our, rtol=1e-6, atol=1e-6)
+    o_s = rg.sample(o_our.cpu().numpy(), 10)
+    assert np.array_equal(o_s, gold['fwd_out']), f'{(o_s != gold["fwd_out"]).sum()} of {o_s.size} sampled outputs differ'
+    np.testing.assert_allclose(rg.sample(d_our.cpu().numpy(), 11), gold['fwd_dy_dx'], rtol=1e-6, atol=1e-6)
     # hash grid type
-    from oracle import ngp_oracle as no
-    offs, pls = no.grid_geometry(3, 8, 2, 2.0, 16, 14, None, False)
-    emb_h = torch.rand(int(offs[-1]), 2, device='cuda') - 0.5
-    offt = torch.from_numpy(offs).cuda()
-    a, b = torch.empty(8, B, 2, device='cuda'), torch.empty(8, B, 2, device='cuda')
-    ref.grid_encode_forward(xt, emb_h, offt, a, B, 3, 2, 8, 1.0, 16, None, 0, False)
-    ours.grid_encode_forward(xt, emb_h, offt, b, B, 3, 2, 8, 1.0, 16, None, 0, False)
-    assert torch.equal(a, b)
+    offs, emb_h = rg.hash_problem()
+    b = torch.empty(8, B, 2, device='cuda')
+    ours.grid_encode_forward(xt, torch.from_numpy(emb_h).cuda(), torch.from_numpy(offs).cuda(), b, B, 3, 2, 8, 1.0, 16, None, 0, False)
+    assert np.array_equal(rg.sample(b.cpu().numpy(), 12), gold['hash_out'])
 
 
-def test_grid_backward_matches_reference_cuda():
-    ref = _ref('_ref_gridencoder')
+def test_grid_backward_matches_reference_cuda(gold):
     from sparsefusion_b200 import _gridencoder as ours
-    geo, x, emb = _grid_problem(B=1 << 16)
+    geo, x, emb = rg.grid_problem(1 << 16)
     B, L, C, D = x.shape[0], geo['L'], geo['C'], 3
     xt, et, off = torch.from_numpy(x).cuda(), emb.cuda(), torch.from_numpy(geo['offsets']).cuda()
-    grad = torch.randn(L, B, C, device='cuda')
-    g_ref, g_our = torch.zeros_like(et), torch.zeros_like(et)
-    ref.grid_encode_backward(grad, xt, et, off, g_ref, B, D, C, L, geo['S'], geo['H'], None, None, 1, False)
+    grad = torch.from_numpy(rg.backward_grad(L, B, C)).cuda()
+    g_our = torch.zeros_like(et)
     ours.grid_encode_backward(grad, xt, et, off, g_our, B, D, C, L, geo['S'], geo['H'], None, None, 1, False)
-    assert torch.allclose(g_ref, g_our, rtol=1e-4, atol=1e-5)      # atomic order differs
-    assert torch.equal(g_ref != 0, g_our != 0)                      # same rows touched
+    gn = g_our.cpu().numpy()
+    np.testing.assert_allclose(rg.sample(gn, 13), gold['bwd_grad'], rtol=1e-4, atol=1e-5)      # atomic order differs
+    assert np.array_equal(np.packbits((gn != 0).reshape(-1)), gold['bwd_touched'])             # same rows touched
 
 
-def test_c_restatement_matches_reference_cuda_grid():
-    ref = _ref('_ref_gridencoder')
+def test_c_restatement_matches_reference_cuda_grid(gold):
     from oracle import ngp_oracle as no
     from sparsefusion_b200 import _lib as lib
-    geo, x, emb = _grid_problem(B=1 << 14)
-    B, L, C, D = x.shape[0], geo['L'], geo['C'], 3
-    xt, et, off = torch.from_numpy(x).cuda(), emb.cuda(), torch.from_numpy(geo['offsets']).cuda()
-    o_ref = torch.empty(L, B, C, device='cuda')
-    ref.grid_encode_forward(xt, et, off, o_ref, B, D, C, L, geo['S'], geo['H'], None, 1, False)
+    geo, x, emb = rg.grid_problem(1 << 14)
+    L = geo['L']
     s = torch.empty(L, device='cuda')
     lib.call('sfb_grid_level_scales', L, float(geo['S']), geo['H'], lib.fptr(s), lib.stream())
     out, _, _ = no.grid_encode_forward(x, emb.numpy(), geo['offsets'], geo['S'], geo['H'], 1, False, False, s.cpu().numpy())
-    diff = np.abs(out - o_ref.cpu().numpy())
+    out = rg.sample(out, 14)
+    diff = np.abs(out - gold['small_fwd_out'])
     print('oracle-vs-reference-CUDA grid forward: max abs diff', diff.max(), 'exact fraction', (diff == 0).mean())
-    np.testing.assert_allclose(out, o_ref.cpu().numpy(), rtol=1e-5, atol=1e-6)
+    np.testing.assert_allclose(out, gold['small_fwd_out'], rtol=1e-5, atol=1e-6)
 
 
-def test_raymarching_operators_match_reference_cuda(golden_dir):
-    ref = _ref('_ref_raymarching')
+def test_raymarching_operators_match_reference_cuda(gold, golden_dir):
     from sparsefusion_b200 import _raymarching as ours
     from oracle import ngp_oracle as no
-    g = np.load(f'{golden_dir}/ngp_march.npz')
-    dev = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    ro, rd = no.camera_rays(no.circle_cameras(8)[2], 128, 128)
-    N = ro.shape[0]
-    rot, rdt, aabb = dev(ro), dev(rd), dev(np.array([-4, -4, -4, 4, 4, 4], np.float32))
-    out = {}
-    for tag, m in (('ref', ref), ('our', ours)):
-        nears, fars = torch.empty(N, device='cuda'), torch.empty(N, device='cuda')
-        m.near_far_from_aabb(rot, rdt, aabb, N, 0.2, nears, fars)
-        M = N * 256
-        xyzs, dirs, deltas = torch.zeros(M, 3, device='cuda'), torch.zeros(M, 3, device='cuda'), torch.zeros(M, 2, device='cuda')
-        rays = torch.empty(N, 3, dtype=torch.int32, device='cuda')
-        counter = torch.zeros(2, dtype=torch.int32, device='cuda')
-        noises = dev(np.random.default_rng(1).random(N, dtype=np.float32))
-        m.march_rays_train(rot, rdt, dev(g['bitfield']), 4.0, 0.0, 256, N, 3, 128, M, nears, fars, xyzs, dirs, deltas, rays, counter, noises)
-        torch.cuda.synchronize()
-        r = rays.cpu().numpy()
-        out[tag] = dict(nears=nears, fars=fars, rays=r[np.argsort(r[:, 0])], counter=counter.cpu().numpy(), xyzs=xyzs, deltas=deltas, rays_t=rays)
-    assert torch.equal(out['ref']['nears'], out['our']['nears']) and torch.equal(out['ref']['fars'], out['our']['fars'])
-    assert np.array_equal(out['ref']['counter'], out['our']['counter'])
-    assert np.array_equal(out['ref']['rays'][:, 2], out['our']['rays'][:, 2]), 'per-ray sample counts differ from the reference CUDA kernel'
+    ro, rd, bitfield, noises = rg.march_problem(golden_dir)
+    our = rg.run_march(ours, ro, rd, bitfield, noises)
+    ref = {k[len('march_'):]: gold[k] for k in gold.files if k.startswith('march_')}
+    assert np.array_equal(ref['nears'], our['nears']) and np.array_equal(ref['fars'], our['fars'])
+    assert np.array_equal(ref['counter'], our['counter'])
+    assert np.array_equal(ref['counts'], our['counts']), 'per-ray sample counts differ from the reference CUDA kernel'
     # oracle counts too
-    _, _, _, rays_o, cnt_o = no.march_rays_train(ro, rd, 4.0, g['bitfield'], 3, 128, out['ref']['nears'].cpu().numpy(), out['ref']['fars'].cpu().numpy(),
-                                                 np.random.default_rng(1).random(N, dtype=np.float32), 0.0, 256)
-    assert np.array_equal(rays_o[:, 2], out['ref']['rays'][:, 2]) and int(cnt_o[0]) == int(out['ref']['counter'][0])
-    # points of a few rays, through each implementation's own rays table
-    xr, xo = out['ref']['xyzs'].cpu().numpy(), out['our']['xyzs'].cpu().numpy()
-    for n in np.random.default_rng(2).choice(N, 128, replace=False):
-        _, o1, c1 = out['ref']['rays'][n]
-        _, o2, c2 = out['our']['rays'][n]
-        np.testing.assert_array_equal(xr[o1:o1 + c1], xo[o2:o2 + c2])
-    # composite forward/backward on the reference's point layout
-    m = int(out['ref']['counter'][0])
-    sig, rgb = torch.rand(m, device='cuda') * 20, torch.rand(m, 3, device='cuda')
-    dl, rays_t = out['ref']['deltas'][:m].contiguous(), out['ref']['rays_t']
-    res = {}
-    for tag, mod in (('ref', ref), ('our', ours)):
-        ws, dp, im = torch.empty(N, device='cuda'), torch.empty(N, device='cuda'), torch.empty(N, 3, device='cuda')
-        mod.composite_rays_train_forward(sig, rgb, dl, rays_t, m, N, 1e-4, ws, dp, im)
-        gs, gc = torch.zeros(m, device='cuda'), torch.zeros(m, 3, device='cuda')
-        gws, gim = torch.ones(N, device='cuda') * 0.3, torch.ones(N, 3, device='cuda') * 0.7
-        mod.composite_rays_train_backward(gws, gim, sig, rgb, dl, rays_t, ws, im, m, N, 1e-4, gs, gc)
-        res[tag] = (ws, dp, im, gs, gc)
-    for a, b in zip(res['ref'], res['our']):
-        assert torch.allclose(a, b, rtol=1e-6, atol=1e-7)
+    _, _, _, rays_o, cnt_o = no.march_rays_train(ro, rd, 4.0, bitfield, 3, 128, ref['nears'], ref['fars'], noises, 0.0, rg.STEPS)
+    assert np.array_equal(rays_o[:, 2], ref['counts']) and int(cnt_o[0]) == int(ref['counter'][0])
+    # points of a few rays, and composite forward / backward keyed by (ray, sample)
+    np.testing.assert_array_equal(our['xyzs'], ref['xyzs'])
+    for k in ('ws', 'depth', 'image', 'grad_sigma', 'grad_rgb'):
+        np.testing.assert_allclose(our[k], ref[k], rtol=1e-6, atol=1e-7, err_msg=k)
     # morton / packbits
-    coords = torch.randint(0, 128, (50000, 3), dtype=torch.int32, device='cuda')
-    i1, i2 = torch.empty(50000, dtype=torch.int32, device='cuda'), torch.empty(50000, dtype=torch.int32, device='cuda')
-    ref.morton3D(coords, 50000, i1)
-    ours.morton3D(coords, 50000, i2)
-    assert torch.equal(i1, i2)
-    grid = torch.randn(3 * 128 ** 3, device='cuda')
-    b1, b2 = torch.empty(3 * 128 ** 3 // 8, dtype=torch.uint8, device='cuda'), torch.empty(3 * 128 ** 3 // 8, dtype=torch.uint8, device='cuda')
-    ref.packbits(grid, b1.numel(), 0.1, b1)
-    ours.packbits(grid, b2.numel(), 0.1, b2)
-    assert torch.equal(b1, b2)
+    i2 = torch.empty(50000, dtype=torch.int32, device='cuda')
+    ours.morton3D(torch.from_numpy(rg.morton_coords()).cuda(), 50000, i2)
+    assert np.array_equal(rg.sample(i2.cpu().numpy(), 15), gold['morton'])
+    b2 = torch.empty(3 * 128 ** 3 // 8, dtype=torch.uint8, device='cuda')
+    ours.packbits(torch.from_numpy(rg.density_grid()).cuda(), b2.numel(), 0.1, b2)
+    assert np.array_equal(rg.sample(b2.cpu().numpy(), 16), gold['packbits'])

@@ -1,4 +1,4 @@
-"""VLDM UNet forward + PLMS sampler on the GPU (tcgen05 TF32 engine) against the oracle and the reference's golden vectors.
+"""VLDM UNet forward + PLMS sampler on the GPU (wgmma TF32 engine) against the oracle and the reference's golden vectors.
 
 Bar (BASELINE.json north_star): relative L2 error <= 1e-3 on the predicted noise, against the fp32 reference.
 """

@@ -1,4 +1,4 @@
-"""SD KL-f8 VAE (SURVEY §8f row 1) on the sm_100a engine against (a) the golden vectors minted from the REFERENCE's own Encoder / Decoder
+"""SD KL-f8 VAE (SURVEY §8f row 1) on the sm_90a engine against (a) the golden vectors minted from the REFERENCE's own Encoder / Decoder
 (tests/golden/vae.npz, oracle/gen_golden.py `vae`) and (b) the torch restatement oracle/vae_oracle.py in fp64 on bigger inputs (tests/test_oracle_vae.py
 pins that restatement to the same golden on CPU).
 

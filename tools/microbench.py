@@ -1,5 +1,5 @@
 """Per-kernel timings on the GPU box (CUDA events, L2 flushed between iterations) -> gpurun_out/microbench.json.
-Used to pick tile/split heuristics and to fill DESIGN.md's per-kernel roofline table; not the headline bench."""
+Used to pick tile/split heuristics; not the headline bench."""
 import json
 import os
 import sys
@@ -195,7 +195,7 @@ def vae_trace(out):
 
 
 def conv_phases(out):
-    """where a tcgen05 conv launch spends its time (sfb_conv_phase_trace): medians over 20 launches, cold L2, arena-style accumulate mode"""
+    """where a wgmma conv launch spends its time (sfb_conv_phase_trace): medians over 20 launches, cold L2, arena-style accumulate mode"""
     global FLUSH
     import numpy as np
     from sparsefusion_b200 import _lib

@@ -1,8 +1,8 @@
-"""gpurun_out/*.csv (ncu exports made on the GPU box by tools/gpu_profile.sh) -> compact per-launch tables under profiles/.
+"""Nsight Compute raw CSV exports (`ncu --page raw --csv`) -> compact per-launch tables under profiles/ (not kept in git).
 
 usage: python tools/summarize_profiles.py r01
 Keeps, per profiled launch: kernel, grid, duration, DRAM bytes read/written, DRAM / L1 / L2 / SM throughput %, occupancy, registers.
-The full reports stay on the GPU box (100 MB); these tables are what DESIGN.md and bench.py's roofline.traffic cite.
+The full reports are large; these tables are what a roofline analysis of the kernels needs.
 """
 import csv
 import os
