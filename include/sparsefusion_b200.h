@@ -243,6 +243,15 @@ int sfb_plms_update(const float* x, const float* e0, const float* e1, const floa
                     float c3, const float* noise, float alpha, float sigma, float alpha_next, float c, float noise_scale, float clip,
                     float* x_prev, float* x0_out, float* e_out, int64_t n, void* stream);
 
+/* One step of DDPM.p_sample with dynamic thresholding (sparsefusion/vldm.py:289-361), B rows of row_len floats (row_len <= 65536):
+ *   e = cond_scale*e_cond + (1-cond_scale)*e_null (e_null may be NULL: e = e_cond);  x0 = (x - sigma*e) / max(alpha,1e-8);
+ *   s = max(torch.quantile(|x0|, percentile, 'linear'), 1) per row, computed exactly;  x0 = clamp(x0, +-s) / s;
+ *   x_prev = alpha_next * (x*(1-c)/alpha + c*x0) + noise_scale * noise.
+ * s_out [B] receives s, x0_out the unthresholded x0; either may be NULL.  x_prev must not alias the inputs. */
+int sfb_ddpm_dynamic_step(const float* x, const float* e_cond, const float* e_null, float cond_scale, const float* noise, float alpha,
+                          float sigma, float alpha_next, float c, float noise_scale, float percentile, int row_len, int B, float* x_prev,
+                          float* s_out, float* x0_out, void* stream);
+
 /* ============================================================================================
  * 4. Fused Instant-NGP field and optimiser   (external/nerf/network_grid.py NeRFNetwork, torch.optim.Adam)
  * ========================================================================================== */

@@ -1382,3 +1382,172 @@ extern "C" int sfb_plms_update(const float* x, const float* e0, const float* e1,
                                                                                  noise_scale, clip, x_prev, x0_out, e_out, n);
     return sfb::check_launch("plms_update");
 }
+
+// ------------------------------------------------------------------------------------ DDPM ancestral step with dynamic thresholding
+// One launch per step of DDPM.p_sample (sparsefusion/vldm.py:289-361) when dynamic_thresholding is on.  Per row (one sample of row_len floats):
+//   e  = cond_scale * e_cond + (1 - cond_scale) * e_null      (classifier-free guidance; e = e_cond when e_null is NULL)
+//   x0 = (x - sigma * e) / max(alpha, 1e-8)
+//   s  = max(torch.quantile(|x0|, p, 'linear'), 1);  x0 = clamp(x0, -s, s) / s
+//   x_prev = alpha_next * (x * (1 - c) / alpha + c * x0) + noise_scale * noise        (same expression order as plms_update_kernel)
+// The quantile is exact: |x0| >= 0, so the order of its uint32 bit patterns is the order of the values, and a 4-pass radix select on 8-bit digits
+// finds the value of rank floor(p * (n - 1)) without sorting; the next rank is either the same value (ties) or the least value above it.  A row
+// is split over a thread-block cluster of up to 8 CTAs (kDynChunk floats each, held in shared memory); their digit histograms are summed
+// through distributed shared memory, as in gn_cluster_kernel.
+namespace sfb {
+constexpr int kDynThreads = 1024;
+constexpr int kDynChunk = 8192;       // floats of a row per CTA: 32 KB of shared memory
+constexpr int kDynMaxCluster = 8;     // portable cluster size: rows up to 65 536 floats (4 x 128 x 128 latents)
+
+template <bool CLUSTER>
+__device__ __forceinline__ void dyn_sync() {
+    if (CLUSTER) cg::this_cluster().sync();
+    else __syncthreads();
+}
+
+template <bool CLUSTER>
+__global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
+    const float* __restrict__ x, const float* __restrict__ e_cond, const float* __restrict__ e_null, float cond_scale,
+    const float* __restrict__ noise, float alpha, float sigma, float alpha_next, float c, float noise_scale, float percentile, int row_len,
+    float* __restrict__ x_prev, float* __restrict__ s_out, float* __restrict__ x0_out) {
+    pdl_sync();
+    extern __shared__ float x0s[];                 // this CTA's slice of the row's x0
+    __shared__ unsigned hist[2][256];              // digit histogram, double-buffered so that one cluster barrier per pass suffices
+    __shared__ unsigned tot[256];
+    __shared__ unsigned sel[3];                    // selected digit, rank left within it, its count
+    __shared__ unsigned vmin;
+    unsigned k = 1, crank = 0;
+    if (CLUSTER) {
+        cg::cluster_group cl = cg::this_cluster();
+        k = cl.num_blocks();
+        crank = cl.block_rank();
+    }
+    const int chunk = (row_len + (int)k - 1) / (int)k;
+    const int i0 = min(row_len, (int)crank * chunk), len = min(row_len, i0 + chunk) - i0;
+    const int64_t base = (int64_t)blockIdx.y * row_len + i0;
+    const int lane = threadIdx.x & 31;
+    for (int i = threadIdx.x; i < 512; i += blockDim.x) (&hist[0][0])[i] = 0u;
+    if (threadIdx.x == 0) vmin = 0xffffffffu;
+
+    const float cn = 1.f - cond_scale;
+    const float alpha_c = fmaxf(alpha, 1e-8f);
+    for (int i = threadIdx.x; i < len; i += blockDim.x) {
+        float e = cond_scale * e_cond[base + i];
+        if (e_null) e += cn * e_null[base + i];
+        const float x0 = (x[base + i] - sigma * e) / alpha_c;
+        x0s[i] = x0;
+        if (x0_out) x0_out[base + i] = x0;
+    }
+
+    // torch.quantile(..., interpolation='linear'): rank = q * (n - 1) in fp32, values at floor / ceil of it, lerp (ATen/native/Lerp.h)
+    const float rk = percentile * (float)(row_len - 1);
+    const int klo = (int)rk, khi = (int)ceilf(rk);
+    const float w = rk - (float)klo;
+    unsigned prefix = 0u, want = (unsigned)klo, cnt_eq = 0u;
+    const int iters = (len + blockDim.x - 1) / blockDim.x;
+#pragma unroll 1
+    for (int pass = 0; pass < 4; ++pass) {
+        const int shift = 24 - 8 * pass;
+        const unsigned pmask = pass == 0 ? 0u : (0xffffffffu << (shift + 8));
+        unsigned* h = hist[pass & 1];
+        __syncthreads();                                           // x0s written, h zeroed
+        for (int it = 0; it < iters; ++it) {                       // warp-uniform trip count: __match_any_sync below needs full warps
+            const int i = it * blockDim.x + threadIdx.x;
+            const unsigned u = i < len ? (__float_as_uint(x0s[i]) & 0x7fffffffu) : 0u;
+            const bool m = i < len && (u & pmask) == prefix;
+            const unsigned d = (u >> shift) & 255u;
+            const unsigned peers = __match_any_sync(0xffffffffu, m ? d : 0xffffffffu);   // lanes with the same digit add once
+            if (m && lane == __ffs(peers) - 1) atomicAdd(&h[d], (unsigned)__popc(peers));
+        }
+        dyn_sync<CLUSTER>();                                       // every CTA's histogram of this pass is complete
+        for (int b = threadIdx.x; b < 256; b += blockDim.x) {
+            unsigned s = 0u;
+            if (CLUSTER) {
+                cg::cluster_group cl = cg::this_cluster();
+                for (unsigned r = 0; r < k; ++r) s += cl.map_shared_rank(h, r)[b];
+            } else {
+                s = h[b];
+            }
+            tot[b] = s;
+        }
+        // every peer finished reading the other buffer before it reached the barrier above: clear it for the next pass
+        for (int b = threadIdx.x; b < 256; b += blockDim.x) hist[(pass + 1) & 1][b] = 0u;
+        __syncthreads();
+        if (threadIdx.x < 32) {                                    // find the digit holding rank `want`: 8 bins per lane, warp prefix sum
+            unsigned v[8], sum = 0u;
+#pragma unroll
+            for (int j = 0; j < 8; ++j) { v[j] = tot[lane * 8 + j]; sum += v[j]; }
+            unsigned incl = sum;
+#pragma unroll
+            for (int o = 1; o < 32; o <<= 1) {
+                const unsigned n = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += n;
+            }
+            unsigned acc = incl - sum;
+            if (want >= acc && want < incl) {
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {
+                    if (want >= acc && want < acc + v[j]) { sel[0] = lane * 8 + j; sel[1] = want - acc; sel[2] = v[j]; }
+                    acc += v[j];
+                }
+            }
+        }
+        __syncthreads();
+        prefix |= sel[0] << shift;
+        want = sel[1];
+        cnt_eq = sel[2];
+    }
+    const float vlo = __uint_as_float(prefix);
+    float vhi = vlo;
+    if (khi != klo && want + 1u >= cnt_eq) {                       // rank khi lies above the ties of vlo: the least |x0| greater than vlo
+        unsigned m = 0xffffffffu;
+        for (int i = threadIdx.x; i < len; i += blockDim.x) {
+            const unsigned u = __float_as_uint(x0s[i]) & 0x7fffffffu;
+            if (u > prefix) m = min(m, u);
+        }
+        m = __reduce_min_sync(0xffffffffu, m);
+        if (lane == 0) atomicMin(&vmin, m);
+        dyn_sync<CLUSTER>();
+        if (CLUSTER) {
+            cg::cluster_group cl = cg::this_cluster();
+            for (unsigned r = 0; r < k; ++r) m = min(m, *cl.map_shared_rank(&vmin, r));
+        } else {
+            m = vmin;
+        }
+        vhi = __uint_as_float(m);
+    }
+    if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");   // done reading the peers' shared memory ...
+    const float dv = vhi - vlo;
+    // lerp(vlo, vhi, w) exactly as ATen/native/Lerp.h compiles for CUDA (the product and the add contract to one fma)
+    const float q = fabsf(w) < 0.5f ? __fmaf_rn(w, dv, vlo) : __fmaf_rn(-dv, 1.f - w, vhi);
+    const float s = fmaxf(q, 1.f);
+    if (s_out && crank == 0 && threadIdx.x == 0) s_out[blockIdx.y] = s;
+    for (int i = threadIdx.x; i < len; i += blockDim.x) {
+        const float x0 = fminf(fmaxf(x0s[i], -s), s) / s;
+        const float xv = x[base + i];
+        const float mean = alpha_next * (xv * (1.f - c) / alpha + c * x0);
+        x_prev[base + i] = mean + noise_scale * noise[base + i];
+    }
+    if (CLUSTER) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // ... and stays resident until the peers are too
+}
+}  // namespace sfb
+
+extern "C" int sfb_ddpm_dynamic_step(const float* x, const float* e_cond, const float* e_null, float cond_scale, const float* noise, float alpha,
+                                     float sigma, float alpha_next, float c, float noise_scale, float percentile, int row_len, int B, float* x_prev,
+                                     float* s_out, float* x0_out, void* stream) {
+    SFB_REQUIRE(B >= 0 && B <= 65535, "ddpm_dynamic_step: B must be 0..65535");
+    if (B == 0) return SFB_OK;
+    SFB_REQUIRE(x && e_cond && noise && x_prev, "ddpm_dynamic_step: null pointer");
+    SFB_REQUIRE(row_len >= 1 && row_len <= sfb::kDynChunk * sfb::kDynMaxCluster, "ddpm_dynamic_step: row_len must be 1..%d", sfb::kDynChunk * sfb::kDynMaxCluster);
+    SFB_REQUIRE(percentile >= 0.f && percentile <= 1.f, "ddpm_dynamic_step: percentile must be in [0, 1]");
+    const unsigned k = (unsigned)((row_len + sfb::kDynChunk - 1) / sfb::kDynChunk);
+    const size_t smem = (size_t)((row_len + (int)k - 1) / (int)k) * sizeof(float);
+    cudaStream_t st = sfb::as_stream(stream);
+    if (k == 1) {
+        SFB_LAUNCH(sfb::ddpm_dynamic_step_kernel<false>, dim3(1, B), sfb::kDynThreads, smem, st, x, e_cond, e_null, cond_scale, noise, alpha, sigma,
+                   alpha_next, c, noise_scale, percentile, row_len, x_prev, s_out, x0_out);
+    } else {
+        SFB_LAUNCH_CLUSTER(sfb::ddpm_dynamic_step_kernel<true>, dim3(k, B), sfb::kDynThreads, smem, st, k, x, e_cond, e_null, cond_scale, noise, alpha,
+                           sigma, alpha_next, c, noise_scale, percentile, row_len, x_prev, s_out, x0_out);
+    }
+    return sfb::check_launch("ddpm_dynamic_step");
+}

@@ -279,8 +279,63 @@ def render_bench(out):
     print('render', out['render'], flush=True)
 
 
+def sample_bench(out):
+    """one DDPM.sample (T = 500, FULL UNet, 32x32 latents) per batch size and guidance scale, and the dynamic-threshold step kernel alone"""
+    import subprocess
+    from sparsefusion_b200 import _lib
+    from sparsefusion_b200.imagen_pytorch import Unet
+    from sparsefusion_b200.vldm import DDPM
+    out['card'] = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                                 text=True).stdout.strip()
+    print('card', out['card'], flush=True)
+    unet = Unet(channels=4, dim=256, dim_mults=(1, 2, 4, 4), num_resnet_blocks=(2, 2, 2, 2), layer_attns=(False, False, False, True),
+                layer_cross_attns=(False,) * 4, cond_images_channels=256, attn_pool_text=False, cond_on_z=False, conditional_embed_dim=None)
+    ddpm = DDPM(channels=4, unets=(unet,), conditional_encoder=None, conditional_embed_dim=None, image_sizes=(32,), timesteps=500, cond_drop_prob=0.1,
+                pred_objectives='noise', conditional=False, auto_normalize_img=False, clip_output=True, dynamic_thresholding=False, clip_value=10).cuda()
+    torch.nn.init.normal_(ddpm.unets[0].get_parameter('final_conv.weight'), std=0.02)
+    out['sample'] = {}
+    for nb in (1, 4, 8):
+        cond = torch.randn(nb, 256, 32, 32, device='cuda')
+        for cs in (1.0, 3.0):
+            run = lambda: ddpm.sample(cond_images=cond, batch_size=nb, cond_scale=cs, use_tqdm=False)
+            run()                                                   # graph capture, time features of the 501 noise levels
+            ts = []
+            for _ in range(2):
+                torch.cuda.synchronize()
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                run()
+                b.record()
+                torch.cuda.synchronize()
+                ts.append(a.elapsed_time(b))
+            rec = dict(sample_ms=round(min(ts), 1), per_step_ms=round(min(ts) / 500, 3), all_ms=[round(t, 1) for t in ts])
+            out['sample'][f'b{nb}_cs{cs:g}'] = rec
+            print('sample', nb, cs, rec, flush=True)
+        if nb == 1:
+            mb = sum(v.numel() * v.element_size() for v in next(iter(ddpm._sampling['time'].values())).values()) / 1e6
+            out['sample']['time_features_mb'] = round(mb, 1)
+            print('sample: time features of the 501 noise levels', round(mb, 1), 'MB', flush=True)
+        r = out['sample'][f'b{nb}_cs3']['sample_ms'] / out['sample'][f'b{nb}_cs1']['sample_ms']
+        out['sample'][f'b{nb}_guidance_ratio'] = round(r, 3)
+        print('sample', nb, 'guided / unguided', round(r, 3), flush=True)
+    out['dynamic_step'] = {}
+    for n in (4096, 65536):
+        for B in (1, 8):
+            x, e, z = (torch.randn(B, n, device='cuda') * 3 for _ in range(3))
+            y = torch.empty_like(x)
+            step = lambda: _lib.call('sfb_ddpm_dynamic_step', _lib.fptr(x), _lib.fptr(e), None, 1.0, _lib.fptr(z), 0.7, 0.7, 0.75, 0.05, 0.1, 0.95,
+                                     n, B, _lib.fptr(y), None, None, _lib.stream())
+            us = timeit(lambda: [step() for _ in range(100)], iters=10, warmup=2, flush=False) * 10.   # ms per 100 launches -> us per launch
+            out['dynamic_step'][f'n{n}_b{B}'] = round(us, 2)
+            print('dynamic_step', n, B, f'{us:.2f} us', flush=True)
+
+
 def main():
     out = {'device': torch.cuda.get_device_name(0), 'conv': [], 'grid': {}}
+    if 'sample' in sys.argv:
+        sample_bench(out)
+        print(json.dumps(out), flush=True)
+        return
     if 'unet' in sys.argv or len(sys.argv) == 1:
         unet_bench(out)
     if 'render' in sys.argv or len(sys.argv) == 1:
