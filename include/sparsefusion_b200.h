@@ -371,6 +371,31 @@ int sfb_seq_attention(const float* qkv, float* out, int S, int B, int E, void* s
 /* in place over n floats (n % 4 == 0): kind 0 ReLU, 1 GELU (erf) */
 int sfb_act_inplace(float* x, int64_t n, int kind, void* stream);
 
+/* ==========================================================================================
+ * section 9 -- mesh extraction from a density lattice (NeRFRenderer.export_mesh, external/nerf/renderer_df.py:121-153)
+ *    Volumes are fp32 [X][Y][Z] row-major (i slowest, k fastest); axis order (i, j, k) = (x, y, z).
+ * ========================================================================================== */
+/* scipy.ndimage.gaussian_filter(v, sigma) with its defaults: three separable passes of exp(-x^2 / 2 sigma^2) taps normalised to sum 1,
+ * radius int(4 sigma + 0.5), mode 'reflect' (half-sample symmetric, folded as often as an axis shorter than the radius needs); fp32 with
+ * fp32 accumulation.  in, out, tmp: X*Y*Z floats, three distinct buffers.  0 < sigma, radius <= 32. */
+int sfb_gaussian_filter3d(const float* in, float* out, float* tmp, int X, int Y, int Z, float sigma, void* stream);
+/* population mean and standard deviation (ddof = 0) of n floats, accumulated in fp64 in a fixed order: out2 [2] doubles = (mean, std).
+ * work: SFB_VOLUME_STATS_WORK doubles of scratch (the per-CTA partial sums). */
+#define SFB_VOLUME_STATS_WORK 1024
+int sfb_volume_mean_std(const float* v, int64_t n, double* out2, double* work, void* stream);
+/* Marching cubes at isovalue iso, in two phases around one host read of the counts.  A corner is below when v <= iso; an edge crosses when
+ * one end is below.  Vertices: one per crossing lattice edge, at p0 + t (p1 - p0), t = (iso - v0) / (v1 - v0), p0 the lower-index end, in
+ * index units; ordered by lattice point (i slowest, k fastest), then owned edge (+i, +j, +k).  Triangles: int32 vertex indices, ordered by
+ * cell (same order) and then the triangle table (sparsefusion_b200/csrc/mc_tables.cuh); each face's normal points toward decreasing value.
+ * Output is a pure function of the volume (no atomics).  Lattices of 1..SFB_MC_MAX_AXIS points per axis.
+ *   scratch: sfb_marching_cubes_scratch_bytes(X, Y, Z) bytes (0 = lattice out of range), shared by the two phases.
+ *   count:   counts [2] int64 (device) <- (V, F).
+ *   emit:    verts [V,3] fp32, tris [F,3] int32 (either may be NULL when its count is 0; V must be below 2^31). */
+#define SFB_MC_MAX_AXIS 1024
+uint64_t sfb_marching_cubes_scratch_bytes(int X, int Y, int Z);
+int sfb_marching_cubes_count(const float* v, int X, int Y, int Z, float iso, void* scratch, int64_t* counts, void* stream);
+int sfb_marching_cubes_emit(const float* v, int X, int Y, int Z, float iso, const void* scratch, float* verts, int32_t* tris, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

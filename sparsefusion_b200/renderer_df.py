@@ -5,7 +5,8 @@ Same class / method names and keyword arguments (``render``, ``render_batched``,
 ``update_extra_state``, ``reset_extra_state``), same result dictionaries, same registered buffers
 (``aabb_train``, ``aabb_infer``, and ``density_grid`` / ``density_bitfield`` / ``step_counter`` with cuda_ray), so
 ``ngp_network.render(rays_o, rays_d, staged=False, perturb=True, bg_color=0, ..., **vars(opt))`` works unchanged.
-``export_mesh`` (offline asset export through mcubes/xatlas) is out of scope (SURVEY.md §2.1 row 7).
+``export_mesh`` runs the reference's mcubes export on the GPU (sparsefusion_b200/mesh.py: lattice query through the fused field kernel,
+Gaussian smoothing, marching cubes, OBJ); the textured xatlas/nvdiffrast export, dead code in the reference, is not provided.
 
 ``run`` is the default path (opt.cuda_ray = False, distillation.py:505).  The reference spells it as ~150 eager
 launches and evaluates the field three times (coarse, fine, colour); here it is seven kernels and every point is
@@ -124,8 +125,23 @@ class NeRFRenderer(nn.Module):
         self.mean_count = 0
         self.local_step = 0
 
-    def export_mesh(self, *a, **k):
-        raise NotImplementedError('export_mesh (mcubes / xatlas asset export) is outside the distillation hot path')
+    @torch.no_grad()
+    def export_mesh(self, path, resolution=None, S=128, *, grid_resolution=128):
+        """renderer_df.py:121-153 on the GPU: sigma on the lattice linspace(-bound, bound, R)^3 (indexing 'ij', queried in slabs of S
+        x-planes), Gaussian smoothing with sigma = 1.5 voxels, marching cubes at mean + 0.25 std of the smoothed volume, and
+        ``{path}/mcubes_mesh.obj`` with vertices in lattice index units, as the reference writes it.  ``resolution`` is accepted and
+        ignored (the reference overrides it with 128); ``grid_resolution`` sets R (128 = the reference's lattice).
+        Returns (verts [V,3] float32 in world units, v / (R-1) * 2 bound - bound; tris [F,3] int32) on the parameters' device.
+        Works with either cuda_ray setting: it reads neither mean_density nor the density bitfield."""
+        import os
+        from . import mesh
+        R = int(grid_resolution)
+        sigma = mesh.density_lattice(self, R, S)
+        smooth = mesh.smooth_gaussian(sigma, 1.5)
+        mean, std = mesh.volume_mean_std(smooth)
+        verts, tris = mesh.marching_cubes(smooth, mean + 0.25 * std)
+        mesh.write_obj(os.path.join(path, 'mcubes_mesh.obj'), verts, tris)
+        return verts / (R - 1) * (2 * self.bound) - self.bound, tris
 
     # ------------------------------------------------------------------------------------------ default path
     def run(self, rays_o, rays_d, num_steps=128, upsample_steps=128, light_d=None, ambient_ratio=1.0, shading='albedo', bg_color=None,

@@ -4,6 +4,7 @@ import json
 import os
 import sys
 
+import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -330,10 +331,78 @@ def sample_bench(out):
             print('dynamic_step', n, B, f'{us:.2f} us', flush=True)
 
 
+def mesh_bench(out):
+    """NeRFRenderer.export_mesh stage by stage at R = 128, 256, 512 (seeded field, +-0.5 embeddings): device-event times of the lattice
+    query, smoothing, statistics (includes the host read of the two doubles), marching-cubes count (includes the host read of V and F) and
+    emit, medians of 5 after one warm-up; the host OBJ write is timed separately (wall clock, to a temporary directory)."""
+    import subprocess
+    import tempfile
+    import time
+    from oracle import ngp_oracle as no
+    from sparsefusion_b200 import _lib, mesh
+    from sparsefusion_b200.network_grid import NeRFNetwork, get_default_torch_ngp_opt
+    out['card'] = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                                 text=True).stdout.strip()
+    print('card', out['card'], flush=True)
+    net = NeRFNetwork(get_default_torch_ngp_opt())
+    sd = net.state_dict()
+    sd.update(no.make_field_params(seed=0))
+    net.load_state_dict(sd)
+    net = net.cuda().eval()
+    out['mesh'] = {}
+
+    def ev(fn):
+        a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        a.record()
+        r = fn()
+        b.record()
+        torch.cuda.synchronize()
+        return r, a.elapsed_time(b)
+
+    with torch.no_grad():
+        for R in (128, 256, 512):
+            rows = []
+            for it in range(6):
+                sig, t_q = ev(lambda: mesh.density_lattice(net, R, 128))
+                sm, t_s = ev(lambda: mesh.smooth_gaussian(sig, 1.5))
+                (mean, std), t_st = ev(lambda: mesh.volume_mean_std(sm))
+                iso = mean + 0.25 * std
+                # the two marching-cubes phases, as mesh.marching_cubes runs them, timed apart
+                nbytes = _lib.load().sfb_marching_cubes_scratch_bytes(R, R, R)
+                scratch = torch.empty(nbytes, dtype=torch.uint8, device='cuda')
+                counts = torch.empty(2, dtype=torch.int64, device='cuda')
+                isof = float(np.float32(iso))
+                (nv, nf), t_c = ev(lambda: (_lib.call('sfb_marching_cubes_count', _lib.fptr(sm), R, R, R, isof, scratch.data_ptr(), counts.data_ptr(),
+                                                      _lib.stream()), counts.tolist())[1])
+                verts = torch.empty(nv, 3, device='cuda')
+                tris = torch.empty(nf, 3, dtype=torch.int32, device='cuda')
+                _, t_e = ev(lambda: _lib.call('sfb_marching_cubes_emit', _lib.fptr(sm), R, R, R, isof, scratch.data_ptr(), verts.data_ptr(),
+                                              tris.data_ptr(), _lib.stream()))
+                with tempfile.TemporaryDirectory() as d:
+                    t0 = time.perf_counter()
+                    mesh.write_obj(os.path.join(d, 'mcubes_mesh.obj'), verts, tris)
+                    t_w = (time.perf_counter() - t0) * 1e3
+                    obj_mb = os.path.getsize(os.path.join(d, 'mcubes_mesh.obj')) / 1e6
+                if it:
+                    rows.append((t_q, t_s, t_st, t_c, t_e, t_w))
+                del sig, sm, scratch
+            med = [float(m) for m in np.median(np.array(rows), axis=0)]
+            gpu = sum(med[:5])
+            rec = dict(field_query_ms=round(med[0], 2), smooth_ms=round(med[1], 2), stats_ms=round(med[2], 2), mc_count_ms=round(med[3], 2),
+                       mc_emit_ms=round(med[4], 2), gpu_total_ms=round(gpu, 2), obj_write_ms=round(med[5], 1), vertices=nv, triangles=nf,
+                       obj_mb=round(obj_mb, 1), gpu_share=round(gpu / (gpu + med[5]), 3))
+            out['mesh'][str(R)] = rec
+            print('mesh', R, rec, flush=True)
+
+
 def main():
     out = {'device': torch.cuda.get_device_name(0), 'conv': [], 'grid': {}}
     if 'sample' in sys.argv:
         sample_bench(out)
+        print(json.dumps(out), flush=True)
+        return
+    if 'mesh' in sys.argv:
+        mesh_bench(out)
         print(json.dumps(out), flush=True)
         return
     if 'unet' in sys.argv or len(sys.argv) == 1:
