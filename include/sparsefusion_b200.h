@@ -242,6 +242,13 @@ int sfb_gate_residual_nhwc(const float* h, int64_t ldh, const float* gate, const
 int sfb_plms_update(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1, float c2,
                     float c3, const float* noise, float alpha, float sigma, float alpha_next, float c, float noise_scale, float clip,
                     float* x_prev, float* x0_out, float* e_out, int64_t n, void* stream);
+/* sfb_plms_update for a batch whose rows follow their own noise schedules (scene-batched sampling, PLMSSampler.sample_rows):
+ * row_scalars [rows][5] = (alpha, sigma, alpha_next, c, noise_scale) of each row's own (t, t_next); every other argument as
+ * sfb_plms_update, with x / eps / noise / outputs holding `rows` contiguous rows of row_len floats (rows <= 65535).  Row r's result is
+ * bit-identical to sfb_plms_update on that row with its scalars. */
+int sfb_plms_update_rows(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1, float c2,
+                         float c3, const float* noise, const float* row_scalars, float clip, float* x_prev, float* x0_out,
+                         int rows, int64_t row_len, void* stream);
 
 /* One step of DDPM.p_sample with dynamic thresholding (sparsefusion/vldm.py:289-361), B rows of row_len floats (row_len <= 65536):
  *   e = cond_scale*e_cond + (1-cond_scale)*e_null (e_null may be NULL: e = e_cond);  x0 = (x - sigma*e) / max(alpha,1e-8);

@@ -1349,25 +1349,54 @@ int sfb_gate_residual_nhwc(const float* h, int64_t ldh, const float* gate, const
 //   x0 = clamp((x - sigma * e') / max(alpha, 1e-8), -clip, clip)  (predict_start_from_noise + clamp, :184,:205)
 //   x_prev = alpha_next * (x * (1 - c) / alpha + c * x0) + noise_scale * noise     (q_posterior mean + sigma_t * z, :208-212)
 // The per-step scalars (alpha, sigma, alpha_next, c, noise_scale = mask * exp(0.5 * log var)) are computed on the host from t, t_next.
+// plms_update_rows_kernel is the same element for a batch whose rows sit at different noise levels (scene-batched sampling): row blockIdx.y reads
+// its five scalars from a table.  Both kernels run plms_update_element, so a row's result is bit-identical to a separate sfb_plms_update launch.
 namespace sfb {
+__device__ __forceinline__ void plms_update_element(int64_t i, const float* __restrict__ x, const float* __restrict__ e0,
+                                                    const float* __restrict__ e1, const float* __restrict__ e2, const float* __restrict__ e3,
+                                                    float c0, float c1, float c2, float c3, const float* __restrict__ noise, float alpha,
+                                                    float sigma, float alpha_next, float c, float noise_scale, float clip,
+                                                    float* __restrict__ x_prev, float* __restrict__ x0_out, float* __restrict__ e_out) {
+    float e = c0 * e0[i];
+    if (e1) e += c1 * e1[i];
+    if (e2) e += c2 * e2[i];
+    if (e3) e += c3 * e3[i];
+    const float xv = x[i];
+    float x0 = (xv - sigma * e) / fmaxf(alpha, 1e-8f);
+    x0 = fminf(fmaxf(x0, -clip), clip);
+    const float mean = alpha_next * (xv * (1.f - c) / alpha + c * x0);
+    x_prev[i] = mean + noise_scale * noise[i];
+    if (x0_out) x0_out[i] = x0;
+    if (e_out) e_out[i] = e;
+}
+
 __global__ void plms_update_kernel(const float* __restrict__ x, const float* __restrict__ e0, const float* __restrict__ e1,
                                    const float* __restrict__ e2, const float* __restrict__ e3, float c0, float c1, float c2, float c3,
                                    const float* __restrict__ noise, float alpha, float sigma, float alpha_next, float c, float noise_scale,
                                    float clip, float* __restrict__ x_prev, float* __restrict__ x0_out, float* __restrict__ e_out, int64_t n) {
     pdl_sync();
-    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
-        float e = c0 * e0[i];
-        if (e1) e += c1 * e1[i];
-        if (e2) e += c2 * e2[i];
-        if (e3) e += c3 * e3[i];
-        const float xv = x[i];
-        float x0 = (xv - sigma * e) / fmaxf(alpha, 1e-8f);
-        x0 = fminf(fmaxf(x0, -clip), clip);
-        const float mean = alpha_next * (xv * (1.f - c) / alpha + c * x0);
-        x_prev[i] = mean + noise_scale * noise[i];
-        if (x0_out) x0_out[i] = x0;
-        if (e_out) e_out[i] = e;
-    }
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
+        plms_update_element(i, x, e0, e1, e2, e3, c0, c1, c2, c3, noise, alpha, sigma, alpha_next, c, noise_scale, clip, x_prev, x0_out, e_out);
+}
+
+__global__ void plms_update_rows_kernel(const float* __restrict__ x, const float* __restrict__ e0, const float* __restrict__ e1,
+                                        const float* __restrict__ e2, const float* __restrict__ e3, float c0, float c1, float c2, float c3,
+                                        const float* __restrict__ noise, const float* __restrict__ row_scalars, float clip,
+                                        float* __restrict__ x_prev, float* __restrict__ x0_out, int64_t row_len) {
+    pdl_sync();
+    __shared__ float s[5];
+    const int64_t off = (int64_t)blockIdx.y * row_len;
+    if (threadIdx.x < 5) s[threadIdx.x] = row_scalars[blockIdx.y * 5 + threadIdx.x];
+    __syncthreads();
+    const float alpha = s[0], sigma = s[1], alpha_next = s[2], c = s[3], noise_scale = s[4];
+    // row-local pointers (NULL stays NULL): element i of the row is element off + i of the batch
+    const float* r1 = e1 ? e1 + off : nullptr;
+    const float* r2 = e2 ? e2 + off : nullptr;
+    const float* r3 = e3 ? e3 + off : nullptr;
+    float* rx0 = x0_out ? x0_out + off : nullptr;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < row_len; i += (int64_t)gridDim.x * blockDim.x)
+        plms_update_element(i, x + off, e0 + off, r1, r2, r3, c0, c1, c2, c3, noise + off, alpha, sigma, alpha_next, c, noise_scale, clip,
+                            x_prev + off, rx0, nullptr);
 }
 }  // namespace sfb
 
@@ -1381,6 +1410,19 @@ extern "C" int sfb_plms_update(const float* x, const float* e0, const float* e1,
     SFB_LAUNCH(sfb::plms_update_kernel, (unsigned)blocks, 256, 0, sfb::as_stream(stream), x, e0, e1, e2, e3, c0, c1, c2, c3, noise, alpha, sigma, alpha_next, c,
                                                                                  noise_scale, clip, x_prev, x0_out, e_out, n);
     return sfb::check_launch("plms_update");
+}
+
+extern "C" int sfb_plms_update_rows(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1,
+                                    float c2, float c3, const float* noise, const float* row_scalars, float clip, float* x_prev, float* x0_out,
+                                    int rows, int64_t row_len, void* stream) {
+    if (rows == 0 || row_len == 0) return SFB_OK;
+    SFB_REQUIRE(x && e0 && noise && row_scalars && x_prev, "plms_update_rows: null pointer");
+    SFB_REQUIRE(rows > 0 && rows <= 65535 && row_len > 0, "plms_update_rows: rows must be in [1, 65535]");
+    int64_t bx = (row_len + 255) / 256;
+    if (bx > 1024) bx = 1024;
+    SFB_LAUNCH(sfb::plms_update_rows_kernel, dim3((unsigned)bx, (unsigned)rows), 256, 0, sfb::as_stream(stream), x, e0, e1, e2, e3, c0, c1, c2, c3,
+               noise, row_scalars, clip, x_prev, x0_out, row_len);
+    return sfb::check_launch("plms_update_rows");
 }
 
 // ------------------------------------------------------------------------------------ DDPM ancestral step with dynamic thresholding

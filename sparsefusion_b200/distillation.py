@@ -24,6 +24,8 @@ Two step semantics:
   step, as many renders as views), the photometric sub-step is computed by one rank (``itr % R``), and the flat 7.46 MB gradient is summed
   with ONE all-reduce per step.  Every random draw of a view (render jitter, inverse-CDF samples, PLMS noise) comes from a generator
   keyed by (seed, iteration, view), so the step's result does not depend on R (up to fp32 summation order).
+* ``MultiSceneDistiller`` / ``distill_scenes`` distil S scenes at once, each on the reference's iteration exactly; only the SDS sub-step's VAE
+  encode, PLMS sampling (``PLMSSampler.sample_rows``: every scene at its own noise level) and decode are batched over the scenes.
 
 ``fusion_substep`` / ``photometric_substep`` with world_size > 1 remain as the one-view-per-rank form (rank r takes entry 1 + r of the
 permutation, all-reduce, Adam with grad_scale 1/R) that ``tests/test_multirank_gpu.py`` pins against the single-rank minibatch.
@@ -81,7 +83,10 @@ def view_seed(seed: int, itr: int, view: int, stream: int) -> int:
 
 class KeyedNoise:
     """``noise_fn`` of the PLMS sampler for a batch of views: row i of every draw comes from view i's own generator (one randn of ``chunk`` draws
-    per view per sampling run, sliced by the sampler's calls), so a view's noise does not depend on which other views share its batch"""
+    per view per sampling run, sliced by the sampler's calls), so a view's noise does not depend on which other views share its batch.
+
+    ``rows`` (``PLMSSampler.sample_rows``): the draw serves only those views, row i of it view ``rows[i]``.  A view left out of a draw has
+    finished its run and may not draw again, so every view still drawing is at the same position of its own stream."""
 
     def __init__(self, seeds, device, chunk: int = 128):
         self.gens = []
@@ -90,14 +95,23 @@ class KeyedNoise:
             g.manual_seed(int(sd))
             self.gens.append(g)
         self.device, self.chunk, self.buf, self.pos = device, chunk, None, 0
+        self.finished = set()
 
-    def __call__(self, like: torch.Tensor) -> torch.Tensor:
-        assert like.shape[0] == len(self.gens), 'KeyedNoise: batch rows must match the views it was keyed for'
+    def __call__(self, like: torch.Tensor, rows=None) -> torch.Tensor:
+        n = len(self.gens)
+        if rows is None:
+            assert like.shape[0] == n, 'KeyedNoise: batch rows must match the views it was keyed for'
+        else:
+            rows = [int(r) for r in rows]
+            assert like.shape[0] == len(rows) and not self.finished & set(rows), 'KeyedNoise: a view that stopped drawing may not draw again'
+            self.finished |= set(range(n)) - set(rows)
         if self.buf is None or self.pos >= self.chunk:
             self.buf = torch.stack([torch.randn(self.chunk, *like.shape[1:], generator=g, device=self.device, dtype=like.dtype) for g in self.gens], dim=1)
             self.pos = 0
         out = self.buf[self.pos]
         self.pos += 1
+        if rows is not None and rows != list(range(n)):
+            out = torch.stack([out[r] for r in rows])        # one launch, no host-to-device index copy
         return out
 
 
@@ -298,30 +312,56 @@ class Distiller:
     def _fusion_substep_fused(self, itr, max_thres, vi, u, feats):
         """the same sub-step with the image-space work in three kernels: bilinear x2 to NCHW (for the VAE), loss value + gradient at full
         resolution, adjoint of the bilinear back to the render's [N,3] / [N] outputs"""
-        c = self.cache
-        img, ws, hw = self._render_raw(c.target_rays_o[vi], c.target_rays_d[vi], 'B')
-        up = glue.upsample2x_render(img.detach(), ws.detach(), hw, hw)                         # :287-288, planes (r, g, b, opacity)
+        img, ws, hw, up = self._fusion_render(vi)
+        pred_img = None
         if itr > self.start_fusion_step:                                                      # :294
-            with torch.no_grad():
-                latents = self.vae.encode(normalize(up[None, :3])).mode() * self.z_scale_factor          # :299
-                if max_thres is None:
-                    max_thres = u.clamp(min=0.0, max=0.99).item()                             # :303
-                pred_x0, _, _, _ = self.sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
-                pred_img = unnormalize(self.vae.decode(1.0 / self.z_scale_factor * pred_x0)).clip(0.0, 1.0)   # :309
-                if self.pred_img_hook is not None:
-                    pred_img = self.pred_img_hook([vi], pred_img)
+            if max_thres is None:
+                max_thres = u.clamp(min=0.0, max=0.99).item()                                 # :303
+            pred_img = self._fusion_target([up], feats, max_thres)
+            if self.pred_img_hook is not None:
+                pred_img = self.pred_img_hook([vi], pred_img)
+            self.last['unet_calls'] = self.sampler.last_unet_calls
+        return self._fusion_apply(itr, img, ws, hw, up, vi, None if pred_img is None else pred_img[0], max_thres)
+
+    # the fused fusion sub-step in three parts, so that MultiSceneDistiller can batch the middle one over scenes
+    def _fusion_render(self, vi, itr=None):
+        """render of target view vi with its x2 bilinear upsampling (:287-288): (image [N,3], weights_sum [N], hw, planes [4,2hw,2hw] (r, g, b,
+        opacity)).  With ``itr`` the render's draws come from the (iteration, view) keyed generator (``_keyed_render``)."""
+        c = self.cache
+        if itr is None:
+            img, ws, hw = self._render_raw(c.target_rays_o[vi], c.target_rays_d[vi], 'B')
+        else:
+            img, ws, hw = self._keyed_render(c.target_rays_o[vi], c.target_rays_d[vi], itr, vi, 1)
+        return img, ws, hw, glue.upsample2x_render(img.detach(), ws.detach(), hw, hw)
+
+    @torch.no_grad()
+    def _fusion_target(self, ups, feats, max_thres, sampler=None, noise_fn=None):
+        """the denoised targets of a batch of upsampled renders: VAE encode (:299), PLMS sampling (:304), decode (:309) -> [B,3,2hw,2hw].
+        ``max_thres`` is one float shared by the batch (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows`` with ``noise_fn``)."""
+        sampler = self.sampler if sampler is None else sampler
+        batch = ups[0][None, :3] if len(ups) == 1 else torch.stack([up[:3] for up in ups])
+        latents = self.vae.encode(normalize(batch)).mode() * self.z_scale_factor                # :299
+        if isinstance(max_thres, (list, tuple)):
+            pred_x0 = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn)[0]
+        else:
+            pred_x0, _, _, _ = sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
+        return unnormalize(self.vae.decode(1.0 / self.z_scale_factor * pred_x0)).clip(0.0, 1.0)     # :309
+
+    def _fusion_apply(self, itr, img, ws, hw, up, vi, pred_img, max_thres):
+        """loss value and gradient (:307-344; SDS against ``pred_img`` [3,2hw,2hw], or the EFT bootstrap when it is None), backward (:345), Adam (:352)"""
+        if pred_img is not None:
             weight = 1.0 - plms_sigmoid(plms_log_snr(float(max_thres)))                      # 1 - alpha_cumprod of the run's first noise level (:307)
             g_extra, percep_term = None, None
             if self.percep is not None and itr >= self.start_percep_step:                     # :176-178, :312-314: value and gradient together
-                pv, pg = self.percep.value_and_grad(up[:3], pred_img[0], normalize=True)
+                pv, pg = self.percep.value_and_grad(up[:3], pred_img, normalize=True)
                 percep_term, g_extra = pv * self.lambda_percep, pg * self.lambda_percep
-            loss, g_img, g_ws = glue.fusion_loss(up, pred_img[0], hw, hw, 'sds', weight, self.lambda_color, self.lambda_sil, self.lambda_opacity,
+            loss, g_img, g_ws = glue.fusion_loss(up, pred_img, hw, hw, 'sds', weight, self.lambda_color, self.lambda_sil, self.lambda_opacity,
                                                  g_extra=g_extra)
             if percep_term is not None:
                 loss = loss + percep_term
-            self.last['unet_calls'] = self.sampler.last_unet_calls
         else:                                                                                 # EFT bootstrap :316-329
-            loss, g_img, g_ws = glue.fusion_loss(up, c.target_eft_image[vi], hw, hw, 'eft', 1.0, self.lambda_color, self.lambda_sil, self.lambda_opacity)
+            loss, g_img, g_ws = glue.fusion_loss(up, self.cache.target_eft_image[vi], hw, hw, 'eft', 1.0, self.lambda_color, self.lambda_sil,
+                                                 self.lambda_opacity)
         torch.autograd.backward((img, ws), (g_img, g_ws))                                     # :345
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))   # :352
         self.last['fusion_loss'] = loss
@@ -438,6 +478,140 @@ class Distiller:
 
 
 # ----------------------------------------------------------------------------------------------------------------------
+# scene-batched distillation: S scenes, each on the reference's iteration, sharing the VAE and UNet batches
+# ----------------------------------------------------------------------------------------------------------------------
+def _keyed_render_noise(seed, itr, view, stream, n, opt, device):
+    """(perturb_noise [n, num_steps], pdf_noise [n, upsample_steps]) from the (seed, iteration, view, stream) keyed generator"""
+    g = torch.Generator(device=device)
+    g.manual_seed(view_seed(seed, itr, view, stream))
+    return (torch.rand(n, opt.num_steps, generator=g, device=device),                  # renderer_df.py:363
+            torch.rand(n, opt.upsample_steps, generator=g, device=device))             # renderer_df.py:31
+
+
+class MultiSceneDistiller:
+    """Distils S scenes at once on one GPU.  Every scene runs the reference's iteration exactly -- photometric sub-step and Adam, then ONE
+    target view and Adam (``Distiller.step`` with ``views_per_step=None``) -- with its own network, optimiser and random streams, held by one
+    ``Distiller`` per scene.  What is shared is the SDS work: the S upsampled renders go through ONE VAE encode, ONE ``PLMSSampler.sample_rows``
+    (each scene at its own noise level, so with its own number of UNet evaluations; the UNet runs at the batch of scenes still sampling) and
+    ONE decode, in chunks of at most ``max_batch`` scenes.  The SDS phase's UNet and VAE run at batch S instead of S times at batch 1.
+
+    Draws of scene k: the view permutation and ``u`` from ``torch.Generator().manual_seed(seeds[k])`` in the reference's order (as in
+    ``Distiller(seed=seeds[k])``); the render jitter / inverse-CDF samples of the photometric render from ``view_seed(seeds[k], itr, 0, 0)``, those
+    of the fusion render of view v from ``view_seed(seeds[k], itr, v, 1)`` and the PLMS noise from ``view_seed(seeds[k], itr, v, 2)``.  A scene's
+    trajectory therefore does not depend on which scenes share its batch.  Parity tests replace them through ``render_noise(scene, 'A'|'B')`` and
+    ``plms_noise(scene) -> noise_fn``, the per-scene counterparts of ``Distiller.render_noise`` and ``PLMSSampler.noise_fn``.
+
+    Not supported: ``views_per_step`` (NotImplementedError), ``fused_glue=False`` and ``opt.hw_scale != 2`` (NotImplementedError), scenes of
+    different image, latent or ray sizes (ValueError), CPU tensors (RuntimeError)."""
+
+    def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, **kw):
+        if kw.get('views_per_step') is not None:
+            raise NotImplementedError('MultiSceneDistiller runs the reference iteration (one target view per scene); views_per_step is not supported')
+        if not kw.get('fused_glue', True) or int(opt.hw_scale) != 2:
+            raise NotImplementedError('MultiSceneDistiller uses the fused image-space kernels (fused_glue=True, hw_scale=2)')
+        if kw.get('world_size', 1) != 1:
+            raise NotImplementedError('MultiSceneDistiller runs on one rank: give each rank its own share of the scenes')
+        if not (len(ngps) == len(caches) == len(seeds)) or len(caches) == 0:
+            raise ValueError(f'MultiSceneDistiller: {len(ngps)} networks, {len(caches)} caches, {len(seeds)} seeds')
+        fields = list(SceneCache.__dataclass_fields__)
+        for c in caches:
+            for f in fields:
+                t = getattr(c, f)
+                if not t.is_cuda:
+                    raise RuntimeError(f'MultiSceneDistiller: SceneCache.{f} must be a CUDA tensor (there is no CPU path)')
+                if tuple(t.shape[1:]) != tuple(getattr(caches[0], f).shape[1:]):
+                    raise ValueError(f'MultiSceneDistiller: scenes differ in SceneCache.{f} size ({tuple(t.shape[1:])} vs '
+                                     f'{tuple(getattr(caches[0], f).shape[1:])}); batched scenes need equal image, latent and ray sizes')
+        self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, **kw) for ngp, cache, sd in zip(ngps, caches, seeds)]
+        self.seeds = [int(s) for s in seeds]
+        self.max_batch = int(max_batch)
+        self.opt = opt
+        lead = self.scenes[0]
+        self.start_fusion_step = lead.start_fusion_step
+        # one sampler for all scenes: its UnetGraph holds one graph per batch size (at most max_batch of them)
+        self.sampler = PLMSSampler(vldm, lead.sampler.plms_steps, use_cuda_graph=lead.sampler.use_cuda_graph)
+        self.render_noise = None   # parity tests: callable(scene, 'A'|'B') -> (perturb_noise, pdf_noise) of that scene's render
+        self.plms_noise = None     # parity tests: callable(scene) -> noise_fn(like) serving that scene's PLMS draws
+        self.last = {}
+
+    def __len__(self):
+        return len(self.scenes)
+
+    def _render_hook(self, k, itr):
+        d = self.scenes[k]
+        if self.render_noise is not None:
+            return lambda w, k=k: self.render_noise(k, w)
+        n, dev = d.cache.input_rays_o.shape[1], d.cache.input_rgb.device
+        return lambda w: _keyed_render_noise(self.seeds[k], itr, 0, 0, n, self.opt, dev)
+
+    def _plms_noise_fn(self, ks, views, itr, dev):
+        """noise_fn of one sample_rows run over scenes ks: row i is scene ks[i]'s own stream"""
+        if self.plms_noise is None:
+            return KeyedNoise([view_seed(self.seeds[k], itr, v, 2) for k, v in zip(ks, views)], dev)
+        fns = [self.plms_noise(k) for k in ks]
+
+        def route(like, rows=None):
+            rows = range(len(ks)) if rows is None else rows
+            return torch.cat([fns[r](like[i:i + 1]) for i, r in enumerate(rows)])
+        return route
+
+    def photometric_substep(self, itr: int):
+        """every scene's photometric sub-step (:185-247) through ``Distiller.photometric_substep``; returns the [S] losses"""
+        out = []
+        for k, d in enumerate(self.scenes):
+            d.render_noise = self._render_hook(k, itr)
+            out.append(d.photometric_substep(itr))
+        return torch.stack(out)
+
+    def fusion_substep(self, itr: int, max_thres: Optional[float] = None):
+        """every scene's fusion sub-step (:259-352) with the VAE encode, PLMS sampling and decode batched over chunks of scenes; returns the [S]
+        losses.  ``max_thres`` forces one noise level for every scene (tests); by default scene k uses its own ``u`` (:303)."""
+        S = len(self.scenes)
+        sds = itr > self.start_fusion_step
+        losses, calls, replays = [None] * S, [0] * S, 0
+        for lo in range(0, S, self.max_batch):
+            ks = list(range(lo, min(S, lo + self.max_batch)))
+            views, mts, renders = [], [], []
+            for k in ks:
+                d, c = self.scenes[k], self.scenes[k].cache
+                d.optimizer.zero_grad()                                                        # :261
+                perm = torch.randperm(c.target_features.shape[0], generator=d.gen)            # :263
+                vi = shard_target_view(perm, 0)                                                # :264
+                u = torch.rand(1, generator=d.gen)                                             # :303
+                views.append(vi)
+                mts.append(float(max_thres) if max_thres is not None else u.clamp(min=0.0, max=0.99).item())
+                if self.render_noise is not None:
+                    d.render_noise_keyed = lambda w, v, k=k: self.render_noise(k, w)
+                renders.append(d._fusion_render(vi, itr))
+            pred = None
+            if sds:
+                dev = renders[0][0].device
+                feats = torch.cat([self.scenes[k].cache.target_features[v:v + 1] for k, v in zip(ks, views)])
+                pred = self.scenes[ks[0]]._fusion_target([r[3] for r in renders], feats, mts, sampler=self.sampler,
+                                                         noise_fn=self._plms_noise_fn(ks, views, itr, dev))
+                replays += self.sampler.last_graph_replays
+                for j, k in enumerate(ks):
+                    calls[k] = self.sampler.last_row_calls[j]
+                    self.scenes[k].last['unet_calls'] = calls[k]
+            for j, k in enumerate(ks):
+                img, ws, hw, up = renders[j]
+                losses[k] = self.scenes[k]._fusion_apply(itr, img, ws, hw, up, views[j], None if pred is None else pred[j], mts[j])
+            del renders
+        if sds:
+            self.last['unet_calls'] = calls
+            self.last['graph_replays'] = replays
+        return torch.stack(losses)
+
+    def step(self, itr: int, max_thres: Optional[float] = None):
+        """one iteration of the reference's loop (distillation.py:174-352) for every scene; returns ([S] photometric, [S] fusion) losses"""
+        with torch.cuda.device(self.scenes[0].cache.input_rgb.device):
+            a = self.photometric_substep(itr)
+            b = self.fusion_substep(itr, max_thres)
+        self.last['photo_loss'], self.last['fusion_loss'] = a, b
+        return a, b
+
+
+# ----------------------------------------------------------------------------------------------------------------------
 # distillation_loop: the reference's entry point (sparsefusion/distillation.py:26-497), same signature
 # ----------------------------------------------------------------------------------------------------------------------
 from .network_grid import NeRFNetwork, get_default_torch_ngp_opt  # noqa: E402,F401  (re-exported: demo.py:9 imports both names from this module)
@@ -545,3 +719,43 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     torch.save({'model_state_dict': ngp_network.state_dict()}, w_addr)
     print('input idx', input_idx)
     return ngp_network
+
+
+def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None):
+    """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
+    one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
+    arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
+    or ``scene_builder.build(...)``), one ``PerceptualLoss`` serves all scenes, scene k is seeded with ``seed + k`` (``seed`` drawn from torch's
+    seed when None), and every network is saved as ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
+    Scenes of one call must share image, latent and ray sizes.  With several GPUs, each rank passes its own share of the scenes.
+    ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  Returns the optimised networks in the order of ``scenes``."""
+    import os
+    from .lpips_vgg import PerceptualLoss
+    eft, vae, vldm = model_tuple
+    exp_dir = getattr(args, 'exp_dir', save_dir)
+    for sc in scenes:
+        os.makedirs(f'{exp_dir}/render_imgs/{sc[0]}/', exist_ok=True)                                                # :57-58
+    os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
+    os.makedirs(save_dir, exist_ok=True)
+    device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
+    builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
+    caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
+              for _, cams, rgb, mask, _, input_idx in scenes]
+    base = torch.seed() % (2 ** 31) if seed is None else int(seed)
+    with torch.cuda.device(device):
+        perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
+        ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
+        msd = MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(scenes))], percep=perceptual_loss,
+                                  plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
+                                  lambda_percep=0.1, start_percep_step=1000)
+        for itr in range(max_itr):                                                                                  # :174
+            if use_diffusion:
+                msd.step(itr)
+            else:
+                msd.photometric_substep(itr)
+            if on_iteration is not None:
+                on_iteration(itr, msd)
+        torch.cuda.synchronize(device)
+    for (seq_name, *_rest), ngp in zip(scenes, ngps):
+        torch.save({'model_state_dict': ngp.state_dict()}, f'{save_dir}/{seq_name}.pt')                             # :495-496
+    return ngps

@@ -395,8 +395,86 @@ def mesh_bench(out):
             print('mesh', R, rec, flush=True)
 
 
+def scenes_bench(out):
+    """scene-batched distillation (MultiSceneDistiller) against the same scenes as S sequential Distiller.step calls, SDS phase: FULL UNet, full
+    VAE, LPIPS on, 32^2 latents, 128^2 rays, S in {1, 2, 4, 8}.  Scene k is seeded k in both arms, so both draw the same u sequence and run the
+    same iterations; the two arms are timed alternately (device events around K iterations, after a warm-up that captures every graph shape)."""
+    import subprocess
+    from bench import build_gpu
+    from sparsefusion_b200.distillation import MultiSceneDistiller, SceneCache
+    from sparsefusion_b200.network_grid import NeRFNetwork
+    from sparsefusion_b200.synthetic import synthetic_scene
+    out['card'] = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                                 text=True).stdout.strip()
+    print('card', out['card'], flush=True)
+    dev = torch.device('cuda', 0)
+    Distiller, models, _, kw = build_gpu(0, 1, dev)
+    vae, vldm, opt, percep = models['vae'], models['vldm'], models['opt'], kw['percep']
+
+    def ngp():
+        n = NeRFNetwork(opt)
+        n.encoder.embeddings.data.uniform_(-0.5, 0.5)
+        return n.to(dev).train()
+    out['scenes'] = {}
+    K, reps, itr0 = 3, 3, 1001
+    for S in (1, 2, 4, 8):
+        caches = [SceneCache(**synthetic_scene(n_target=8, seed=k)).to(dev) for k in range(S)]
+        torch.cuda.synchronize()
+        mem0 = torch.cuda.memory_reserved()
+        msd = MultiSceneDistiller([ngp() for _ in range(S)], vae, vldm, opt, caches, seeds=list(range(S)), percep=percep, max_batch=8)
+        seq = [Distiller(ngp(), vae, vldm, opt, caches[k], seed=k, percep=percep) for k in range(S)]
+        for d in seq[1:]:
+            d.sampler = seq[0].sampler                                     # one graph per shape for the sequential arm too
+        # capture every batch size 1..S of the batched arm: S distinct run lengths
+        with torch.no_grad():
+            lat = torch.randn(S, 4, 32, 32, device=dev)
+            feats = torch.cat([c.target_features[:1] for c in caches])
+            msd.sampler.sample_rows(lat, [0.99 - 0.1 * k for k in range(S)], feats)
+        torch.cuda.synchronize()
+        graph_mb = (torch.cuda.memory_reserved() - mem0) / 1e6
+        itr = itr0
+        for _ in range(2):                                                 # warm-up
+            msd.step(itr)
+            for d in seq:
+                d.step(itr)
+            itr += 1
+        torch.cuda.synchronize()
+        torch.cuda.reset_peak_memory_stats()
+        tb, ts, rows, replays = [], [], 0, 0
+        for _ in range(reps):
+            for arm, times in (('batched', tb), ('sequential', ts)):
+                a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                a.record()
+                for i in range(K):
+                    if arm == 'batched':
+                        msd.step(itr + i)
+                        rows += sum(msd.last['unet_calls'])
+                        replays += msd.last['graph_replays']
+                    else:
+                        for d in seq:
+                            d.step(itr + i)
+                b.record()
+                torch.cuda.synchronize()
+                times.append(a.elapsed_time(b) / K)
+            itr += K
+        mb, ms = float(np.median(tb)), float(np.median(ts))
+        rec = dict(batched_ms_per_iteration=round(mb, 1), sequential_ms_per_iteration=round(ms, 1), batched_scene_its_per_s=round(S * 1e3 / mb, 2),
+                   sequential_scene_its_per_s=round(S * 1e3 / ms, 2), speedup=round(ms / mb, 3), batched_all_ms=[round(t, 1) for t in tb],
+                   sequential_all_ms=[round(t, 1) for t in ts], unet_rows_per_iteration=round(rows / (K * reps), 1),
+                   graph_replays_per_iteration=round(replays / (K * reps), 1), graph_capture_mb=round(graph_mb, 1),
+                   peak_allocated_gb=round(torch.cuda.max_memory_allocated() / 1e9, 2))
+        out['scenes'][str(S)] = rec
+        print('scenes', S, rec, flush=True)
+        del msd, seq, caches
+        torch.cuda.empty_cache()
+
+
 def main():
     out = {'device': torch.cuda.get_device_name(0), 'conv': [], 'grid': {}}
+    if 'scenes' in sys.argv:
+        scenes_bench(out)
+        print(json.dumps(out), flush=True)
+        return
     if 'sample' in sys.argv:
         sample_bench(out)
         print(json.dumps(out), flush=True)
