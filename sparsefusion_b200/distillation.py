@@ -212,29 +212,45 @@ class Distiller:
         self.render_noise_keyed = None   # parity tests (minibatch step): callable('A'|'B', view) -> the same pair for that view
         self.plms_noise = None     # parity tests (minibatch step): callable(views) -> noise_fn for that batch, replacing KeyedNoise
         self.pred_img_hook = None  # parity tests (minibatch step): callable(views, pred_img) -> pred_img, e.g. to inject a fixed denoised target
+        self._keyed = False        # MultiSceneDistiller: the reference step draws from the keyed generators too (``_render_draws``)
         self.last = {}
 
     # ------------------------------------------------------------------------------------------------
-    def _render_raw(self, rays_o, rays_d, which='A'):
-        """(image [N,3], weights_sum [N], hw) with the autograd graph of the render attached"""
-        kw = self.render_kw
-        if self.render_noise is not None:
-            pn, un = self.render_noise(which)
-            kw = dict(kw, perturb_noise=pn, pdf_noise=un)
+    def _render_draws(self, rays_o, itr, view, stream, keyed):
+        """(perturb_noise [N, num_steps], pdf_noise [N, upsample_steps]) of one render -- stream 0: photometric, 1: fusion -- or None, which
+        lets the renderer draw from torch's global generator as the reference does.  ``keyed`` (the view-batched step, MultiSceneDistiller's
+        scenes): ``render_noise_keyed`` or the (seed, itr, view, stream) generator; otherwise ``render_noise``."""
+        which = 'AB'[stream]
+        if not keyed:
+            return None if self.render_noise is None else self.render_noise(which)
+        if self.render_noise_keyed is not None:
+            return self.render_noise_keyed(which, view)
+        n, dev = rays_o.shape[0], rays_o.device
+        g = torch.Generator(device=dev)
+        g.manual_seed(view_seed(self.seed, itr, view, stream))
+        return (torch.rand(n, self.opt.num_steps, generator=g, device=dev),             # renderer_df.py:363
+                torch.rand(n, self.opt.upsample_steps, generator=g, device=dev))        # renderer_df.py:31
+
+    def _render(self, rays_o, rays_d, draws):
+        """(image [N,3], weights_sum [N], hw) with the autograd graph of the render attached; ``draws`` from ``_render_draws``"""
+        kw = self.render_kw if draws is None else dict(self.render_kw, perturb_noise=draws[0], pdf_noise=draws[1])
         out = self.ngp.render(rays_o[None], rays_d[None], **kw)
         n = rays_o.shape[0]
         return out['image'].reshape(n, 3), out['weights_sum'].reshape(n), int(round(n ** 0.5))
 
-    def _render(self, rays_o, rays_d, which='A'):
-        kw = self.render_kw
-        if self.render_noise is not None:
-            pn, un = self.render_noise(which)
-            kw = dict(kw, perturb_noise=pn, pdf_noise=un)
-        out = self.ngp.render(rays_o[None], rays_d[None], **kw)
-        hw = int(round(rays_o.shape[0] ** 0.5))
-        image = out['image'].reshape(1, hw, hw, 3).permute(0, 3, 1, 2).contiguous()           # :210
-        sil = out['weights_sum'].reshape(1, hw, hw, 1).permute(0, 3, 1, 2).contiguous()       # :211
-        return image, sil
+    def _render_nchw(self, rays_o, rays_d, draws):
+        """the render as the eager path uses it: image [1,3,hw,hw] and silhouette [1,1,hw,hw] (:210-211)"""
+        img, ws, hw = self._render(rays_o, rays_d, draws)
+        return img.reshape(1, hw, hw, 3).permute(0, 3, 1, 2).contiguous(), ws.reshape(1, hw, hw, 1).permute(0, 3, 1, 2).contiguous()
+
+    def _photometric_grad(self, idx, draws):
+        """photometric term of input view idx with the fused kernels: render, loss value and gradient (:216-234), backward; returns the loss"""
+        c = self.cache
+        img, ws, hw = self._render(c.input_rays_o[idx], c.input_rays_d[idx], draws)
+        loss, g_img, g_ws = glue.photometric_loss(img.detach(), ws.detach(), c.input_rgb[idx], c.input_mask[idx], hw, hw, int(self.opt.hw_scale),
+                                                  self.lambda_color, self.lambda_sil, self.lambda_opacity)
+        torch.autograd.backward((img, ws), (g_img, g_ws))
+        return loss
 
     def photometric_substep(self, itr: int):
         """distillation.py:185-247"""
@@ -244,32 +260,28 @@ class Distiller:
         self.ngp.train()
         if self.opt.cuda_ray and itr % 16 == 0:                                               # :181-182
             self.ngp.update_extra_state()
+        draws = self._render_draws(c.input_rays_o[idx], itr, 0, 0, self._keyed)              # keyed: view 0, whichever input view is drawn
         if self.fused_glue:
-            img, ws, hw = self._render_raw(c.input_rays_o[idx], c.input_rays_d[idx], 'A')
-            loss, g_img, g_ws = glue.photometric_loss(img.detach(), ws.detach(), c.input_rgb[idx], c.input_mask[idx], hw, hw, int(self.opt.hw_scale),
-                                                      self.lambda_color, self.lambda_sil, self.lambda_opacity)        # :216-234 value + gradient
             self.optimizer.zero_grad()                                                        # :244
-            torch.autograd.backward((img, ws), (g_img, g_ws))
-            self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))
-            self.optimizer.scheduler_step()                                                   # :247
-            self.last['photo_loss'] = loss
-            return loss
-        image, sil = self._render(c.input_rays_o[idx], c.input_rays_d[idx], 'A')
-        scale = 1.0 / self.opt.hw_scale
-        batch_rgb = F.interpolate(c.input_rgb[idx:idx + 1], scale_factor=scale)               # :216 (nearest)
-        batch_mask = F.interpolate(c.input_mask[idx:idx + 1], scale_factor=scale)             # :217
-        color_err = huber(image, batch_rgb).abs().mean()                                      # :218
-        sil_err = huber(sil, batch_mask).abs().mean()                                         # :222
-        loss = self.lambda_color * color_err + self.lambda_sil * sil_err                      # :227
-        opacity = torch.sqrt(sil ** 2 + .01).mean()                                           # :233
-        loss = loss + self.lambda_opacity * opacity                                           # :234
-        self.optimizer.zero_grad()                                                            # :244
-        loss.backward()
+            loss = self._photometric_grad(idx, draws)
+        else:
+            image, sil = self._render_nchw(c.input_rays_o[idx], c.input_rays_d[idx], draws)
+            scale = 1.0 / self.opt.hw_scale
+            batch_rgb = F.interpolate(c.input_rgb[idx:idx + 1], scale_factor=scale)           # :216 (nearest)
+            batch_mask = F.interpolate(c.input_mask[idx:idx + 1], scale_factor=scale)         # :217
+            color_err = huber(image, batch_rgb).abs().mean()                                  # :218
+            sil_err = huber(sil, batch_mask).abs().mean()                                     # :222
+            loss = self.lambda_color * color_err + self.lambda_sil * sil_err                  # :227
+            opacity = torch.sqrt(sil ** 2 + .01).mean()                                       # :233
+            loss = loss + self.lambda_opacity * opacity                                       # :234
+            self.optimizer.zero_grad()                                                        # :244
+            loss.backward()
+            loss = loss.detach()
         # replicated sub-step: for N>1 the reduce only removes atomic-order drift so that ranks stay bit-identical
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))
         self.optimizer.scheduler_step()                                                       # :247
-        self.last['photo_loss'] = loss.detach()
-        return loss.detach()
+        self.last['photo_loss'] = loss
+        return loss
 
     def fusion_substep(self, itr: int, max_thres: Optional[float] = None):
         """distillation.py:259-352; rank r takes the (1 + r)-th entry of the step's permutation (the reference takes entry 1, :264)"""
@@ -282,18 +294,14 @@ class Distiller:
         feats = c.target_features[vi:vi + 1]
         if self.fused_glue and int(self.opt.hw_scale) == 2:
             return self._fusion_substep_fused(itr, max_thres, vi, u, feats)
-        image, sil = self._render(c.target_rays_o[vi], c.target_rays_d[vi], 'B')
+        image, sil = self._render_nchw(c.target_rays_o[vi], c.target_rays_d[vi], self._render_draws(c.target_rays_o[vi], itr, vi, 1, self._keyed))
         image = F.interpolate(image, scale_factor=self.opt.hw_scale, mode='bilinear')         # :287
         sil = F.interpolate(sil, scale_factor=self.opt.hw_scale, mode='bilinear')             # :288
         if itr > self.start_fusion_step:                                                      # :294
-            with torch.no_grad():
-                latents = self.vae.encode(normalize(image)).mode() * self.z_scale_factor      # :299
-                if max_thres is None:
-                    max_thres = u.clamp(min=0.0, max=0.99).item()                             # :303
-                pred_x0, x_noisy, noise, alpha_cumprod = self.sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True,
-                                                                             max_thres=max_thres)            # :304
-                fusion_weight = (1 - alpha_cumprod).to(pred_x0.device)                        # :307
-                pred_img = unnormalize(self.vae.decode(1.0 / self.z_scale_factor * pred_x0)).clip(0.0, 1.0)   # :309
+            if max_thres is None:
+                max_thres = u.clamp(min=0.0, max=0.99).item()                                 # :303
+            pred_img, alpha_cumprod = self._fusion_target([image[0]], feats, max_thres, None)
+            fusion_weight = (1 - alpha_cumprod).to(pred_img.device)                           # :307 (the sampler's fp32 value)
             fusion_loss = (fusion_weight * (image - pred_img).abs().mean()).sum()             # :310 ([1]-shaped in the reference)
             if self.percep is not None and itr >= self.start_percep_step:                     # :176-178, :312-314
                 fusion_loss = fusion_loss + self.percep(image, pred_img, normalize=True).mean() * self.lambda_percep
@@ -310,45 +318,63 @@ class Distiller:
         return loss.detach()
 
     def _fusion_substep_fused(self, itr, max_thres, vi, u, feats):
-        """the same sub-step with the image-space work in three kernels: bilinear x2 to NCHW (for the VAE), loss value + gradient at full
-        resolution, adjoint of the bilinear back to the render's [N,3] / [N] outputs"""
-        img, ws, hw, up = self._fusion_render(vi)
-        pred_img = None
-        if itr > self.start_fusion_step:                                                      # :294
-            if max_thres is None:
-                max_thres = u.clamp(min=0.0, max=0.99).item()                                 # :303
-            pred_img = self._fusion_target([up], feats, max_thres)
-            if self.pred_img_hook is not None:
-                pred_img = self.pred_img_hook([vi], pred_img)
-            self.last['unet_calls'] = self.sampler.last_unet_calls
-        return self._fusion_apply(itr, img, ws, hw, up, vi, None if pred_img is None else pred_img[0], max_thres)
+        """the same sub-step on target view vi (conditioning ``feats``) with the fused image-space kernels, then Adam (:352)"""
+        if itr > self.start_fusion_step and max_thres is None:
+            max_thres = u.clamp(min=0.0, max=0.99).item()                                     # :303
+        loss = self._fusion_views(itr, [vi], feats, max_thres, self._keyed, 1.0)[0]
+        self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))   # :352
+        self.last['fusion_loss'] = loss
+        return loss
 
-    # the fused fusion sub-step in three parts, so that MultiSceneDistiller can batch the middle one over scenes
-    def _fusion_render(self, vi, itr=None):
-        """render of target view vi with its x2 bilinear upsampling (:287-288): (image [N,3], weights_sum [N], hw, planes [4,2hw,2hw] (r, g, b,
-        opacity)).  With ``itr`` the render's draws come from the (iteration, view) keyed generator (``_keyed_render``)."""
+    def _fusion_views(self, itr, views, feats, max_thres, keyed, scale):
+        """fusion term of target views ``views`` (conditioning ``feats``, read in the SDS phase only) with the image-space work in three kernels
+        (bilinear x2 to NCHW for the VAE, loss value + gradient at full resolution, adjoint of the bilinear back to the render's [N,3] / [N]
+        outputs): renders, ONE SDS target batch passed through ``pred_img_hook`` (or the EFT bootstrap), each view's gradient scaled by
+        ``scale``.  PLMS draws: keyed per view (``plms_noise`` or ``KeyedNoise``) when ``keyed``, else the sampler's own.  Returns the views'
+        losses, unscaled; the caller steps the optimiser."""
+        renders = self._fusion_renders(itr, views, keyed)
+        pred = [None] * len(views)
+        if itr > self.start_fusion_step:                                                      # :294
+            noise_fn = None
+            if keyed:
+                noise_fn = self.plms_noise(views) if self.plms_noise is not None else KeyedNoise([view_seed(self.seed, itr, v, 2) for v in views],
+                                                                                                 renders[0][0].device)
+            pred = self._fusion_target([r[3] for r in renders], feats, max_thres, noise_fn)[0]
+            if self.pred_img_hook is not None:
+                pred = self.pred_img_hook(views, pred)
+            self.last['unet_calls'] = self.sampler.last_unet_calls
+        return [self._fusion_grad(itr, *r, v, p, max_thres, scale) for r, v, p in zip(renders, views, pred)]
+
+    def _fusion_renders(self, itr, views, keyed):
+        """renders of target views (:274-277), then their x2 bilinear upsampling (:287-288): [(image [N,3], weights_sum [N], hw, planes
+        [4,2hw,2hw] (r, g, b, opacity))]"""
         c = self.cache
-        if itr is None:
-            img, ws, hw = self._render_raw(c.target_rays_o[vi], c.target_rays_d[vi], 'B')
-        else:
-            img, ws, hw = self._keyed_render(c.target_rays_o[vi], c.target_rays_d[vi], itr, vi, 1)
-        return img, ws, hw, glue.upsample2x_render(img.detach(), ws.detach(), hw, hw)
+        renders = [self._render(c.target_rays_o[v], c.target_rays_d[v], self._render_draws(c.target_rays_o[v], itr, v, 1, keyed)) for v in views]
+        return [(img, ws, hw, glue.upsample2x_render(img.detach(), ws.detach(), hw, hw)) for img, ws, hw in renders]
 
     @torch.no_grad()
-    def _fusion_target(self, ups, feats, max_thres, sampler=None, noise_fn=None):
-        """the denoised targets of a batch of upsampled renders: VAE encode (:299), PLMS sampling (:304), decode (:309) -> [B,3,2hw,2hw].
-        ``max_thres`` is one float shared by the batch (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows`` with ``noise_fn``)."""
+    def _fusion_target(self, images, feats, max_thres, noise_fn, sampler=None):
+        """the denoised targets of a batch of renders ([C>=3,H,W] each, colour first): VAE encode (:299), PLMS sampling (:304), decode (:309).
+        Returns (pred_img [B,3,H,W], alpha_cumprod [B] of the run's first noise level, fp32).  ``max_thres`` is one float shared by the batch
+        (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows``); ``noise_fn`` serves the run's draws, None: the sampler's own."""
         sampler = self.sampler if sampler is None else sampler
-        batch = ups[0][None, :3] if len(ups) == 1 else torch.stack([up[:3] for up in ups])
+        batch = images[0][None, :3] if len(images) == 1 else torch.stack([im[:3] for im in images])
         latents = self.vae.encode(normalize(batch)).mode() * self.z_scale_factor                # :299
         if isinstance(max_thres, (list, tuple)):
-            pred_x0 = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn)[0]
+            out = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn)
         else:
-            pred_x0, _, _, _ = sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
-        return unnormalize(self.vae.decode(1.0 / self.z_scale_factor * pred_x0)).clip(0.0, 1.0)     # :309
+            prev = sampler.noise_fn
+            if noise_fn is not None:
+                sampler.noise_fn = noise_fn
+            try:
+                out = sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
+            finally:
+                sampler.noise_fn = prev
+        return unnormalize(self.vae.decode(1.0 / self.z_scale_factor * out[0])).clip(0.0, 1.0), out[3]     # :309
 
-    def _fusion_apply(self, itr, img, ws, hw, up, vi, pred_img, max_thres):
-        """loss value and gradient (:307-344; SDS against ``pred_img`` [3,2hw,2hw], or the EFT bootstrap when it is None), backward (:345), Adam (:352)"""
+    def _fusion_grad(self, itr, img, ws, hw, up, vi, pred_img, max_thres, scale=1.0):
+        """loss value and gradient of target view vi (:307-344; SDS against ``pred_img`` [3,2hw,2hw], or the EFT bootstrap when it is None),
+        backward (:345) of the gradient times ``scale``; returns the loss.  The caller steps the optimiser (:352)."""
         if pred_img is not None:
             weight = 1.0 - plms_sigmoid(plms_log_snr(float(max_thres)))                      # 1 - alpha_cumprod of the run's first noise level (:307)
             g_extra, percep_term = None, None
@@ -362,9 +388,9 @@ class Distiller:
         else:                                                                                 # EFT bootstrap :316-329
             loss, g_img, g_ws = glue.fusion_loss(up, self.cache.target_eft_image[vi], hw, hw, 'eft', 1.0, self.lambda_color, self.lambda_sil,
                                                  self.lambda_opacity)
+        if scale != 1.0:
+            g_img, g_ws = g_img * scale, g_ws * scale
         torch.autograd.backward((img, ws), (g_img, g_ws))                                     # :345
-        self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))   # :352
-        self.last['fusion_loss'] = loss
         return loss
 
     def step(self, itr: int, max_thres: Optional[float] = None):
@@ -377,19 +403,6 @@ class Distiller:
         return a, b
 
     # ------------------------------------------------------------------------------------------------ view-batched step (SURVEY.md §8e)
-    def _keyed_render(self, rays_o, rays_d, itr, view, stream):
-        """render with this (iteration, view)'s own jitter / inverse-CDF draws"""
-        n = rays_o.shape[0]
-        if self.render_noise_keyed is not None:
-            pn, un = self.render_noise_keyed(('A', 'B')[stream], view)
-        else:
-            g = torch.Generator(device=rays_o.device)
-            g.manual_seed(view_seed(self.seed, itr, view, stream))
-            pn = torch.rand(n, self.opt.num_steps, generator=g, device=rays_o.device)            # renderer_df.py:363
-            un = torch.rand(n, self.opt.upsample_steps, generator=g, device=rays_o.device)       # renderer_df.py:31
-        out = self.ngp.render(rays_o[None], rays_d[None], **dict(self.render_kw, perturb_noise=pn, pdf_noise=un))
-        return out['image'].reshape(n, 3), out['weights_sum'].reshape(n), int(round(n ** 0.5))
-
     def minibatch_step(self, itr: int, max_thres: Optional[float] = None):
         """one optimiser step on (photometric view + V target views); returns (photometric loss, mean fusion loss) as device scalars.  With
         world_size R each rank handles views[r::R]; the losses returned are the GLOBAL ones only on the rank(s) that computed every term --
@@ -398,7 +411,6 @@ class Distiller:
             raise NotImplementedError('the view-batched step uses the fused image-space kernels (fused_glue=True, hw_scale=2)')
         c = self.cache
         V, R, r = int(self.views_per_step), self.world_size, self.rank
-        dev = c.input_rgb.device
         n_in, n_t = c.input_rgb.shape[0], c.target_features.shape[0]
         idx = int(torch.randperm(n_in, generator=self.gen)[0])                                 # :185-186
         perm = torch.randperm(n_t, generator=self.gen)                                         # :263
@@ -407,68 +419,24 @@ class Distiller:
         mine = shard_views(views, r, R)
         self.ngp.train()
         self.optimizer.zero_grad()
-        zero = torch.zeros((), device=dev)
-        loss_a = zero
+        loss_a = loss_b = torch.zeros((), device=c.input_rgb.device)
+        if self.opt.cuda_ray and itr % 16 == 0:
+            self.ngp.update_extra_state()
         # ---- photometric term: one rank (round-robin over iterations), gradient joins the step's single all-reduce
         if itr % R == r:
-            if self.opt.cuda_ray and itr % 16 == 0:
-                self.ngp.update_extra_state()
-            img, ws, hw = self._keyed_render(c.input_rays_o[idx], c.input_rays_d[idx], itr, idx, 0)
-            loss_a, g_img, g_ws = glue.photometric_loss(img.detach(), ws.detach(), c.input_rgb[idx], c.input_mask[idx], hw, hw, int(self.opt.hw_scale),
-                                                        self.lambda_color, self.lambda_sil, self.lambda_opacity)
-            torch.autograd.backward((img, ws), (g_img, g_ws))
-        elif self.opt.cuda_ray and itr % 16 == 0:
-            self.ngp.update_extra_state()
-        # ---- fusion term over this rank's views, in batches of at most max_batch
+            loss_a = self._photometric_grad(idx, self._render_draws(c.input_rays_o[idx], itr, idx, 0, True))
+        # ---- fusion term over this rank's views, in batches of at most max_batch, gradient = mean over the step's V views
         sds = itr > self.start_fusion_step
         if sds and max_thres is None:
             max_thres = u.clamp(min=0.0, max=0.99).item()
-        loss_b = zero
-        calls = 0
+        if sds and not mine:                               # a rank with no views this step (V < R); otherwise _fusion_views sets it
+            self.last['unet_calls'] = 0
         inv_v = 1.0 / V
         for lo in range(0, len(mine), self.max_batch):
             chunk = mine[lo:lo + self.max_batch]
-            renders = [self._keyed_render(c.target_rays_o[v], c.target_rays_d[v], itr, v, 1) for v in chunk]
-            hw = renders[0][2]
-            ups = [glue.upsample2x_render(im.detach(), w.detach(), hw, hw) for im, w, _ in renders]          # :287-288
-            if sds:
-                with torch.no_grad():
-                    batch = torch.stack([up[:3] for up in ups])                                               # [b,3,256,256]
-                    latents = self.vae.encode(normalize(batch)).mode() * self.z_scale_factor                 # :299
-                    feats = c.target_features[chunk] if isinstance(c.target_features, torch.Tensor) else torch.cat([c.target_features[v:v + 1] for v in chunk])
-                    prev_fn = self.sampler.noise_fn
-                    if self.plms_noise is None:
-                        self.sampler.noise_fn = KeyedNoise([view_seed(self.seed, itr, v, 2) for v in chunk], dev)
-                    else:
-                        self.sampler.noise_fn = self.plms_noise(chunk)
-                    try:
-                        pred_x0, _, _, _ = self.sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
-                    finally:
-                        self.sampler.noise_fn = prev_fn
-                    pred_img = unnormalize(self.vae.decode(1.0 / self.z_scale_factor * pred_x0)).clip(0.0, 1.0)   # :309
-                    if self.pred_img_hook is not None:
-                        pred_img = self.pred_img_hook(chunk, pred_img)
-                calls = self.sampler.last_unet_calls
-                weight = 1.0 - plms_sigmoid(plms_log_snr(float(max_thres)))                                  # :307
-            for j, v in enumerate(chunk):
-                im, w, _ = renders[j]
-                if sds:
-                    g_extra, percep_term = None, None
-                    if self.percep is not None and itr >= self.start_percep_step:                             # :176-178, :312-314
-                        pv, pg = self.percep.value_and_grad(ups[j][:3], pred_img[j], normalize=True)
-                        percep_term, g_extra = pv * self.lambda_percep, pg * self.lambda_percep
-                    lv, g_img, g_ws = glue.fusion_loss(ups[j], pred_img[j], hw, hw, 'sds', weight, self.lambda_color, self.lambda_sil,
-                                                       self.lambda_opacity, g_extra=g_extra)
-                    if percep_term is not None:
-                        lv = lv + percep_term
-                else:
-                    lv, g_img, g_ws = glue.fusion_loss(ups[j], c.target_eft_image[v], hw, hw, 'eft', 1.0, self.lambda_color, self.lambda_sil,
-                                                       self.lambda_opacity)
-                torch.autograd.backward((im, w), (g_img * inv_v, g_ws * inv_v))                               # mean over the step's V views
+            feats = c.target_features[chunk] if sds else None         # cache fields take int, one-row slice or list indices (bench.py's staged cache)
+            for lv in self._fusion_views(itr, chunk, feats, max_thres, True, inv_v):
                 loss_b = loss_b + lv * inv_v
-            del renders, ups
-        if sds:
-            self.last['unet_calls'] = calls
         self.optimizer.sync_grads(R, self.pg)              # the step's ONE collective: sum of every rank's (photometric + fusion) gradient
         self.optimizer.step(grad_scale=1.0)
         self.optimizer.scheduler_step()                                                        # :247
@@ -480,14 +448,6 @@ class Distiller:
 # ----------------------------------------------------------------------------------------------------------------------
 # scene-batched distillation: S scenes, each on the reference's iteration, sharing the VAE and UNet batches
 # ----------------------------------------------------------------------------------------------------------------------
-def _keyed_render_noise(seed, itr, view, stream, n, opt, device):
-    """(perturb_noise [n, num_steps], pdf_noise [n, upsample_steps]) from the (seed, iteration, view, stream) keyed generator"""
-    g = torch.Generator(device=device)
-    g.manual_seed(view_seed(seed, itr, view, stream))
-    return (torch.rand(n, opt.num_steps, generator=g, device=device),                  # renderer_df.py:363
-            torch.rand(n, opt.upsample_steps, generator=g, device=device))             # renderer_df.py:31
-
-
 class MultiSceneDistiller:
     """Distils S scenes at once on one GPU.  Every scene runs the reference's iteration exactly -- photometric sub-step and Adam, then ONE
     target view and Adam (``Distiller.step`` with ``views_per_step=None``) -- with its own network, optimiser and random streams, held by one
@@ -523,26 +483,31 @@ class MultiSceneDistiller:
                     raise ValueError(f'MultiSceneDistiller: scenes differ in SceneCache.{f} size ({tuple(t.shape[1:])} vs '
                                      f'{tuple(getattr(caches[0], f).shape[1:])}); batched scenes need equal image, latent and ray sizes')
         self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, **kw) for ngp, cache, sd in zip(ngps, caches, seeds)]
+        for d in self.scenes:
+            d._keyed = True
         self.seeds = [int(s) for s in seeds]
         self.max_batch = int(max_batch)
-        self.opt = opt
         lead = self.scenes[0]
         self.start_fusion_step = lead.start_fusion_step
         # one sampler for all scenes: its UnetGraph holds one graph per batch size (at most max_batch of them)
         self.sampler = PLMSSampler(vldm, lead.sampler.plms_steps, use_cuda_graph=lead.sampler.use_cuda_graph)
-        self.render_noise = None   # parity tests: callable(scene, 'A'|'B') -> (perturb_noise, pdf_noise) of that scene's render
+        self.render_noise = None
         self.plms_noise = None     # parity tests: callable(scene) -> noise_fn(like) serving that scene's PLMS draws
         self.last = {}
 
     def __len__(self):
         return len(self.scenes)
 
-    def _render_hook(self, k, itr):
-        d = self.scenes[k]
-        if self.render_noise is not None:
-            return lambda w, k=k: self.render_noise(k, w)
-        n, dev = d.cache.input_rays_o.shape[1], d.cache.input_rgb.device
-        return lambda w: _keyed_render_noise(self.seeds[k], itr, 0, 0, n, self.opt, dev)
+    @property
+    def render_noise(self):
+        """parity tests: callable(scene, 'A'|'B') -> (perturb_noise, pdf_noise) of that scene's render, in place of its keyed draws"""
+        return self._render_noise
+
+    @render_noise.setter
+    def render_noise(self, fn):
+        self._render_noise = fn
+        for k, d in enumerate(self.scenes):
+            d.render_noise_keyed = None if fn is None else (lambda which, view, k=k: fn(k, which))
 
     def _plms_noise_fn(self, ks, views, itr, dev):
         """noise_fn of one sample_rows run over scenes ks: row i is scene ks[i]'s own stream"""
@@ -557,11 +522,7 @@ class MultiSceneDistiller:
 
     def photometric_substep(self, itr: int):
         """every scene's photometric sub-step (:185-247) through ``Distiller.photometric_substep``; returns the [S] losses"""
-        out = []
-        for k, d in enumerate(self.scenes):
-            d.render_noise = self._render_hook(k, itr)
-            out.append(d.photometric_substep(itr))
-        return torch.stack(out)
+        return torch.stack([d.photometric_substep(itr) for d in self.scenes])
 
     def fusion_substep(self, itr: int, max_thres: Optional[float] = None):
         """every scene's fusion sub-step (:259-352) with the VAE encode, PLMS sampling and decode batched over chunks of scenes; returns the [S]
@@ -580,22 +541,20 @@ class MultiSceneDistiller:
                 u = torch.rand(1, generator=d.gen)                                             # :303
                 views.append(vi)
                 mts.append(float(max_thres) if max_thres is not None else u.clamp(min=0.0, max=0.99).item())
-                if self.render_noise is not None:
-                    d.render_noise_keyed = lambda w, v, k=k: self.render_noise(k, w)
-                renders.append(d._fusion_render(vi, itr))
-            pred = None
+                renders += d._fusion_renders(itr, [vi], True)
+            pred = [None] * len(ks)
             if sds:
-                dev = renders[0][0].device
                 feats = torch.cat([self.scenes[k].cache.target_features[v:v + 1] for k, v in zip(ks, views)])
-                pred = self.scenes[ks[0]]._fusion_target([r[3] for r in renders], feats, mts, sampler=self.sampler,
-                                                         noise_fn=self._plms_noise_fn(ks, views, itr, dev))
+                pred = self.scenes[ks[0]]._fusion_target([r[3] for r in renders], feats, mts, self._plms_noise_fn(ks, views, itr, renders[0][0].device),
+                                                         sampler=self.sampler)[0]
                 replays += self.sampler.last_graph_replays
                 for j, k in enumerate(ks):
                     calls[k] = self.sampler.last_row_calls[j]
                     self.scenes[k].last['unet_calls'] = calls[k]
             for j, k in enumerate(ks):
-                img, ws, hw, up = renders[j]
-                losses[k] = self.scenes[k]._fusion_apply(itr, img, ws, hw, up, views[j], None if pred is None else pred[j], mts[j])
+                d = self.scenes[k]
+                losses[k] = d.last['fusion_loss'] = d._fusion_grad(itr, *renders[j], views[j], pred[j], mts[j])
+                d.optimizer.step()                                                             # :352 (one rank: grad_scale 1)
             del renders
         if sds:
             self.last['unet_calls'] = calls
@@ -688,35 +647,17 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ones; loss_fn_vgg only feeds the debug metrics).  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
     torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``.
     Returns the optimised network."""
-    import os
     eft, vae, vldm = model_tuple
-    exp_dir = getattr(args, 'exp_dir', save_dir)
-    os.makedirs(f'{exp_dir}/render_imgs/{seq_name}/', exist_ok=True)                                               # :57-58
-    os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
-    os.makedirs(save_dir, exist_ok=True)
-    device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
-    builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
-    cache = builder.build(eft, scene_cameras, scene_rgb, scene_mask, input_idx, use_diffusion=use_diffusion)
-    from .lpips_vgg import PerceptualLoss
-    with torch.cuda.device(device):
-        perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
-        ngp_network = NeRFNetwork(opt).to(device).train()                                                          # :164
-        rank, world = 0, 1
-        if process_group is not None:
-            rank, world = torch.distributed.get_rank(process_group), torch.distributed.get_world_size(process_group)
-        dist = Distiller(ngp_network, vae, vldm, opt, cache.to(device), plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0,   # :148-160
-                         lambda_opacity=1e-3, seed=torch.seed() % (2 ** 31) if seed is None else seed, rank=rank, world_size=world,
-                         process_group=process_group, percep=perceptual_loss, lambda_percep=0.1, start_percep_step=1000, views_per_step=views_per_step)
-        for itr in range(max_itr):                                                                                  # :174
-            if use_diffusion:
-                dist.step(itr)
-            else:
-                dist.photometric_substep(itr)
-            if on_iteration is not None:
-                on_iteration(itr, dist)
-        torch.cuda.synchronize(device)
-    w_addr = f'{save_dir}/{seq_name}.pt'                                                                            # :495-496
-    torch.save({'model_state_dict': ngp_network.state_dict()}, w_addr)
+    rank, world = 0, 1
+    if process_group is not None:
+        rank, world = torch.distributed.get_rank(process_group), torch.distributed.get_world_size(process_group)
+
+    def make(ngps, caches, percep, seed):
+        return Distiller(ngps[0], vae, vldm, opt, caches[0], plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0,   # :148-160
+                         lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
+                         start_percep_step=1000, views_per_step=views_per_step)
+    ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
+                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration)
     print('input idx', input_idx)
     return ngp_network
 
@@ -729,9 +670,21 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     seed when None), and every network is saved as ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
     Scenes of one call must share image, latent and ray sizes.  With several GPUs, each rank passes its own share of the scenes.
     ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  Returns the optimised networks in the order of ``scenes``."""
+    eft, vae, vldm = model_tuple
+
+    def make(ngps, caches, percep, base):
+        return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
+                                   plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
+                                   lambda_percep=0.1, start_percep_step=1000)
+    return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration)
+
+
+def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration):
+    """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
+    ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
+    ``max_itr`` iterations and one checkpoint per scene.  Returns the networks."""
     import os
     from .lpips_vgg import PerceptualLoss
-    eft, vae, vldm = model_tuple
     exp_dir = getattr(args, 'exp_dir', save_dir)
     for sc in scenes:
         os.makedirs(f'{exp_dir}/render_imgs/{sc[0]}/', exist_ok=True)                                                # :57-58
@@ -741,20 +694,17 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
     caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
               for _, cams, rgb, mask, _, input_idx in scenes]
-    base = torch.seed() % (2 ** 31) if seed is None else int(seed)
     with torch.cuda.device(device):
         perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
         ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
-        msd = MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(scenes))], percep=perceptual_loss,
-                                  plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
-                                  lambda_percep=0.1, start_percep_step=1000)
+        dist = make(ngps, caches, perceptual_loss, torch.seed() % (2 ** 31) if seed is None else int(seed))
         for itr in range(max_itr):                                                                                  # :174
             if use_diffusion:
-                msd.step(itr)
+                dist.step(itr)
             else:
-                msd.photometric_substep(itr)
+                dist.photometric_substep(itr)
             if on_iteration is not None:
-                on_iteration(itr, msd)
+                on_iteration(itr, dist)
         torch.cuda.synchronize(device)
     for (seq_name, *_rest), ngp in zip(scenes, ngps):
         torch.save({'model_state_dict': ngp.state_dict()}, f'{save_dir}/{seq_name}.pt')                             # :495-496

@@ -2,7 +2,8 @@
 
 (1) sfb_plms_update_rows is bit-identical to one sfb_plms_update launch per row;
 (2) sample_rows with six different noise levels in one call equals six single-scene sample() runs fed the same per-scene noise;
-(3) MultiSceneDistiller.step equals one Distiller.step per scene with the same injected draws (reduced scenes, both phases, LPIPS in the SDS one);
+(3) MultiSceneDistiller.step equals one Distiller.step per scene with the same injected draws (reduced scenes, both phases, LPIPS in the SDS one),
+    and without injected draws equals Distiller.step fed each scene's (seed, iteration, view)-keyed draws;
 (4) the same at full size (FULL UNet, full VAE, LPIPS, 128^2 rays), 4 scenes, one SDS step;
 (5) distill_scenes writes every scene's checkpoint in the reference layout.
 """
@@ -143,27 +144,47 @@ def _draws(S, n_rays):
              for w in 'AB'} for _ in range(S)]
 
 
+def _keyed_replay(d, itr):
+    """route the draws MultiSceneDistiller keys by view_seed -- photometric (view 0, stream 0), fusion (vi, 1), PLMS (vi, 2) -- through the
+    reference step's hooks of Distiller d"""
+    from sparsefusion_b200.distillation import KeyedNoise, shard_target_view, view_seed
+    g = torch.Generator().manual_seed(d.seed)                   # d.gen's draws of this step, replayed: randperm(n_in), randperm(n_t)
+    torch.randperm(d.cache.input_rgb.shape[0], generator=g)
+    vi = shard_target_view(torch.randperm(d.cache.target_features.shape[0], generator=g), 0)
+    n = d.cache.input_rays_o.shape[1]
+
+    def pair(view, stream):
+        gg = torch.Generator(device='cuda')
+        gg.manual_seed(view_seed(d.seed, itr, view, stream))
+        return (torch.rand(n, d.opt.num_steps, generator=gg, device='cuda'), torch.rand(n, d.opt.upsample_steps, generator=gg, device='cuda'))
+    d.render_noise = lambda w: pair(0, 0) if w == 'A' else pair(vi, 1)
+    d.sampler.noise_fn = KeyedNoise([view_seed(d.seed, itr, vi, 2)], 'cuda')
+
+
 def _single_step(models, cache, k, itr, draws, seed):
-    """Distiller.step of scene k with the injected draws; returns (losses, flat parameters)"""
+    """Distiller.step of scene k with the injected draws (None: MultiSceneDistiller's keyed ones); returns (losses, flat parameters)"""
     from oracle import unet_oracle as uo
     from sparsefusion_b200.distillation import Distiller
     from sparsefusion_b200.network_grid import get_default_torch_ngp_opt
     vae, ddpm, pl = models
     d = Distiller(_ngp(k), vae, ddpm, get_default_torch_ngp_opt(), cache, seed=seed, percep=pl)
-    src = uo.NoiseSource(seed=50 + k)
-    d.sampler.noise_fn = lambda t: src(t.cpu()).to(t.device)
-    d.render_noise = lambda w: draws[w]
+    if draws is None:
+        _keyed_replay(d, itr)
+    else:
+        src = uo.NoiseSource(seed=50 + k)
+        d.sampler.noise_fn = lambda t: src(t.cpu()).to(t.device)
+        d.render_noise = lambda w: draws[w]
     la, lb = d.step(itr)
     return (la.item(), lb.item()), d.optimizer.flat.clone(), d.last.get('unet_calls')
 
 
-def _compare(S, itr, full):
+def _compare(S, itr, full, injected=True):
     from oracle import unet_oracle as uo
     from sparsefusion_b200.distillation import MultiSceneDistiller
     from sparsefusion_b200.network_grid import get_default_torch_ngp_opt
     models = _full_models() if full else _small_models(percep=itr > 1000)
     caches = _scenes(S, full)
-    draws = _draws(S, caches[0].input_rays_o.shape[1])
+    draws = _draws(S, caches[0].input_rays_o.shape[1]) if injected else [None] * S
     seeds = [11 + k for k in range(S)]
     # run-to-run spread of Distiller.step itself: the field backward accumulates with atomics
     ref = [_single_step(models, caches[k], k, itr, draws[k], seeds[k]) for k in range(S)]
@@ -172,9 +193,10 @@ def _compare(S, itr, full):
     spread_l = max(abs(a - b) / abs(b) for a, b in zip(again[0], ref[0][0]))
     vae, ddpm, pl = models
     msd = MultiSceneDistiller([_ngp(k) for k in range(S)], vae, ddpm, get_default_torch_ngp_opt(), caches, seeds=seeds, percep=pl)
-    srcs = [uo.NoiseSource(seed=50 + k) for k in range(S)]
-    msd.render_noise = lambda k, w: draws[k][w]
-    msd.plms_noise = lambda k: (lambda t: srcs[k](t.cpu()).to(t.device))
+    if injected:
+        srcs = [uo.NoiseSource(seed=50 + k) for k in range(S)]
+        msd.render_noise = lambda k, w: draws[k][w]
+        msd.plms_noise = lambda k: (lambda t: srcs[k](t.cpu()).to(t.device))
     la, lb = msd.step(itr)
     print(f'itr {itr}, {S} scenes: Distiller.step run-to-run spread: parameters {spread_p:.2e}, losses {spread_l:.2e}; '
           f'UNet evaluations per scene {msd.last.get("unet_calls")}, graph replays {msd.last.get("graph_replays")}')
@@ -192,6 +214,12 @@ def _compare(S, itr, full):
 @pytest.mark.parametrize('itr', [5, 1500])
 def test_multiscene_step_matches_per_scene_distillers(itr):
     _compare(3, itr, full=False)
+
+
+def test_multiscene_default_draws_are_keyed_by_scene_seed_iteration_and_view():
+    """no hooks: each scene draws from view_seed(seed, itr, 0, 0) (photometric), (vi, 1) (fusion render) and (vi, 2) (PLMS), replayed here
+    through a Distiller's hooks"""
+    _compare(3, 1500, full=False, injected=False)
 
 
 @pytest.mark.timeout(1200)
