@@ -403,6 +403,23 @@ uint64_t sfb_marching_cubes_scratch_bytes(int X, int Y, int Z);
 int sfb_marching_cubes_count(const float* v, int X, int Y, int Z, float iso, void* scratch, int64_t* counts, void* stream);
 int sfb_marching_cubes_emit(const float* v, int X, int Y, int Z, float iso, const void* scratch, float* verts, int32_t* tris, void* stream);
 
+/* ==========================================================================================
+ * section 10 -- image metrics of a scored scene (sparsefusion/distillation.py:391-443 via utils/common_utils.py:48-64: scikit-image SSIM / PSNR)
+ *    Images are fp32 [B][H][W][3] (a render's image [H*W,3] in row-major pixel order, so no transposes).
+ * ========================================================================================== */
+/* SSIM and mean squared error of B image pairs (a[b], b[b]) -> out [2B] doubles:
+ *   out[2b]     skimage.metrics.structural_similarity(a, b, channel_axis=-1, data_range=1) as scikit-image >= 0.19 computes it for float32
+ *               input: per channel, 7x7 uniform window (scipy.ndimage.uniform_filter, mode 'reflect': half-sample symmetric), sample
+ *               covariance (49/48), C1 = 0.01^2, C2 = 0.03^2, the SSIM map in fp32 and its mean in fp64 over the interior (3 pixels cropped
+ *               from every side); the three channel values are stored as fp32 and averaged in fp32, so the value is an fp32 number.
+ *               Window sums are taken in fp64 and rounded to fp32 after each 1D pass, as scipy's line buffers do.
+ *   out[2b+1]   mean of (a - b)^2 over every pixel and channel: fp32 differences and squares, fp64 sum (PSNR = 10 log10(1 / mse)).
+ * Two launches: one CTA per (image, 32x32 output tile) writes four fp64 partial sums to work, then one CTA per image adds them in a fixed
+ * order; no atomics, so repeated calls are bit-identical.  B >= 1, H >= 7, W >= 7 (scikit-image rejects a window larger than the image).
+ *   work: sfb_image_ssim_psnr_work(B, H, W) doubles (0 = sizes rejected). */
+uint64_t sfb_image_ssim_psnr_work(int B, int H, int W);
+int sfb_image_ssim_psnr(const float* a, const float* b, int B, int H, int W, double* out, double* work, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

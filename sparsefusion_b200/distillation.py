@@ -74,7 +74,8 @@ def shard_views(views: list, rank: int, world_size: int) -> list:
 
 
 def view_seed(seed: int, itr: int, view: int, stream: int) -> int:
-    """seed of the generator that serves ONE (iteration, view, stream) -- stream 0: photometric render, 1: fusion render, 2: PLMS noise.
+    """seed of the generator that serves ONE (iteration, view, stream) -- stream 0: photometric render, 1: fusion render, 2: PLMS noise, 3: evaluation
+    render (``evaluate.evaluate_scene``, with iteration 0).
     Keyed draws make a minibatch step independent of how its views are spread over ranks."""
     x = (seed * 0x9E3779B97F4A7C15 + itr * 0xBF58476D1CE4E5B9 + view * 0x94D049BB133111EB + stream * 0xD6E8FEB86659FD93) & 0xFFFFFFFFFFFFFFFF
     x ^= x >> 31
@@ -633,19 +634,48 @@ class ReferenceSceneBuilder:
                           target_features=torch.cat(feats) if feats else empty(256, 32, 32), target_eft_image=torch.cat(eft_imgs) if eft_imgs else empty(3, 256, 256),
                           target_rays_o=torch.stack(t_o) if t_o else empty(n_rays, 3), target_rays_d=torch.stack(t_d) if t_d else empty(n_rays, 3))
 
+    def eval_views(self, scene_cameras, scene_rgb, scene_mask):
+        """the views the reference scores the distilled scene on (:393-406): every scene camera in the voxel frame (:70) through the 256x256
+        ``sampler_grid`` (:85), with ``scene_rgb`` / ``scene_mask`` as ground truth -> ``evaluate.EvalViews``"""
+        try:
+            from utils.camera_utils import RelativeCameraLoader
+            from utils.render_utils import init_ray_sampler
+        except ImportError as e:
+            raise RuntimeError('distillation_loop(evaluate=True) needs the reference tree (utils/camera_utils.py, utils/render_utils.py) and pytorch3d '
+                               'on sys.path to turn pytorch3d cameras into rays; pass a scene_builder with its own eval_views') from e
+        from einops import rearrange
+        from .evaluate import EvalViews
+        relative_cam = RelativeCameraLoader(relative=True, center_at_origin=True)
+        relative_cam_no_origin = RelativeCameraLoader(relative=True, center_at_origin=False)
+        scene_cameras_vox = relative_cam_no_origin.get_relative_camera(scene_cameras, query_idx=[0], center_at_origin=False)   # :70
+        cam_dist_mean = torch.mean(torch.linalg.norm(scene_cameras.get_camera_center(), axis=1))                     # :82-84
+        sampler_grid = init_ray_sampler(self.gpu, 256, 256, min=cam_dist_mean - 5.0, max=cam_dist_mean + 5.0, scale_factor=2)[0]   # :85
+        o, d = [], []
+        for ci in range(len(scene_cameras_vox)):                                                                    # :395-402
+            rb = sampler_grid(relative_cam.get_camera_slice(scene_cameras_vox, [ci]))
+            o.append(rearrange(rb.origins, 'b h w c -> b (h w) c')[0].contiguous())
+            d.append(rearrange(rb.directions, 'b h w c -> b (h w) c')[0].contiguous())
+        return EvalViews(rays_o=torch.stack(o), rays_d=torch.stack(d), rgb=scene_rgb.float(), mask=scene_mask.float())
+
 
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
-                      process_group=None):
+                      process_group=None, evaluate=False):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
 
-    Not reproduced: the matplotlib loss plots and the periodic / final visualisation renders, gifs and debug metrics (:355-388, :391-493) -- logging,
-    outside the hot path; ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference
-    makes).  ``scene_valid_region`` and ``loss_fn_vgg`` are accepted and unused, as in the reference's loop body (:192-195 overwrites the region with
-    ones; loss_fn_vgg only feeds the debug metrics).  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
-    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``.
+    ``evaluate=True`` adds the reference's scene scores (:391-443): before the first iteration the builder's ``eval_views(scene_cameras, scene_rgb,
+    scene_mask)`` gives the views (a ``scene_builder`` without it fails then, not after the loop); after the loop ``evaluate.evaluate_scene`` renders
+    every view in eval mode (jitter keyed by the scene's seed) and scores it with PSNR, SSIM and LPIPS-VGG on the GPU, and
+    ``{save_dir}/metrics/{seq_name}.txt`` is written in the reference's format.  LPIPS uses ``loss_fn_vgg``'s weights (an ``lpips.LPIPS``, as
+    demo.py:33 passes it, or a ``PerceptualLoss``); without it the LPIPS entry is nan rather than a distance from random VGG weights.
+
+    Not reproduced: the matplotlib loss plots, the periodic / final visualisation renders and gifs (:355-388, :444-493) -- logging, outside the
+    hot path; ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference makes).
+    ``scene_valid_region`` is accepted and unused, as in the reference's loop body (:192-195 overwrites the region with ones), and so is
+    ``loss_fn_vgg`` unless ``evaluate``.  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
+    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     rank, world = 0, 1
@@ -657,47 +687,58 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
                          start_percep_step=1000, views_per_step=views_per_step)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
-                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration)
+                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg)
     print('input idx', input_idx)
     return ngp_network
 
 
-def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None):
+def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
+                   evaluate=False, loss_fn_vgg=None):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
     or ``scene_builder.build(...)``), one ``PerceptualLoss`` serves all scenes, scene k is seeded with ``seed + k`` (``seed`` drawn from torch's
     seed when None), and every network is saved as ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
     Scenes of one call must share image, latent and ray sizes.  With several GPUs, each rank passes its own share of the scenes.
-    ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  Returns the optimised networks in the order of ``scenes``."""
+    ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  ``evaluate`` / ``loss_fn_vgg``: each scene is scored and its
+    ``{save_dir}/metrics/{seq_name}.txt`` written as ``distillation_loop(evaluate=True)`` does, scene k's render jitter keyed by ``seed + k``.
+    Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
 
     def make(ngps, caches, percep, base):
         return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000)
-    return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration)
+    return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
+                             loss_fn_vgg)
 
 
-def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration):
+def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
+                      loss_fn_vgg=None):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
-    ``max_itr`` iterations and one checkpoint per scene.  Returns the networks."""
+    ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files (scene k seeded ``seed + k``).
+    Returns the networks."""
     import os
     from .lpips_vgg import PerceptualLoss
+    builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
+    if evaluate and not callable(getattr(builder, 'eval_views', None)):
+        raise TypeError(f'evaluate=True needs the scene builder to provide eval_views(scene_cameras, scene_rgb, scene_mask); '
+                        f'{type(builder).__name__} has none')
     exp_dir = getattr(args, 'exp_dir', save_dir)
     for sc in scenes:
         os.makedirs(f'{exp_dir}/render_imgs/{sc[0]}/', exist_ok=True)                                                # :57-58
     os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
     os.makedirs(save_dir, exist_ok=True)
     device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
-    builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
+    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate else None
     caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
               for _, cams, rgb, mask, _, input_idx in scenes]
     with torch.cuda.device(device):
         perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
         ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
-        dist = make(ngps, caches, perceptual_loss, torch.seed() % (2 ** 31) if seed is None else int(seed))
+        base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
+        dist = make(ngps, caches, perceptual_loss, base_seed)
         for itr in range(max_itr):                                                                                  # :174
             if use_diffusion:
                 dist.step(itr)
@@ -708,4 +749,13 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
         torch.cuda.synchronize(device)
     for (seq_name, *_rest), ngp in zip(scenes, ngps):
         torch.save({'model_state_dict': ngp.state_dict()}, f'{save_dir}/{seq_name}.pt')                             # :495-496
+    if evaluate:
+        from .evaluate import evaluate_scene, write_scene_metrics
+        with torch.cuda.device(device):
+            eval_percep = None if loss_fn_vgg is None else PerceptualLoss('vgg', device=device).load_state_dict(loss_fn_vgg.state_dict())
+            for k, ((seq_name, *_rest), ngp, views) in enumerate(zip(scenes, ngps, eval_views)):
+                scores = evaluate_scene(ngp, views, opt, eval_percep, seed=base_seed + k)                           # :391-433
+                print('warning: this metric is used for debugging only and not the final metric')
+                print(f'{getattr(args, "category", "")} scene {seq_name}')
+                write_scene_metrics(f'{save_dir}/metrics/{seq_name}.txt', scores)                                  # :434-441
     return ngps

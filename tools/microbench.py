@@ -469,8 +469,90 @@ def scenes_bench(out):
         torch.cuda.empty_cache()
 
 
+def eval_bench(out):
+    """scene scoring (sparsefusion_b200.evaluate): sfb_image_ssim_psnr alone at B = 1 and 32 on 256^2 pairs (CUDA events around 50 calls,
+    after a warm-up), and evaluate_scene over 32 views at 256^2 of a seeded field split into its render, LPIPS and SSIM / PSNR parts (device
+    events around each part of one view loop, medians of 5 after a warm-up)."""
+    import subprocess
+    from oracle import ngp_oracle as no
+    from sparsefusion_b200 import evaluate as ev
+    from sparsefusion_b200.distillation import view_seed
+    from sparsefusion_b200.lpips_vgg import PerceptualLoss
+    from sparsefusion_b200.network_grid import NeRFNetwork, get_default_torch_ngp_opt
+    from sparsefusion_b200.synthetic import camera_rays, circle_cameras
+    out['card'] = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                                 text=True).stdout.strip()
+    print('card', out['card'], flush=True)
+    out['eval'] = {}
+    g = torch.Generator(device='cuda').manual_seed(0)
+    for B in (1, 32):
+        a = torch.rand(B, 256, 256, 3, device='cuda', generator=g)
+        b = (a + 0.1 * torch.rand(B, 256, 256, 3, device='cuda', generator=g)).clamp(0, 1)
+        for _ in range(5):
+            ev.image_metrics(a, b)
+        torch.cuda.synchronize()
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for _ in range(50):
+            ev.image_metrics(a, b)
+        t1.record()
+        torch.cuda.synchronize()
+        us = t0.elapsed_time(t1) / 50 * 1e3
+        rec = dict(us_per_call=round(us, 1), us_per_image=round(us / B, 2), input_gbs=round(2 * a.numel() * 4 / (us * 1e3), 1))
+        out['eval'][f'ssim_psnr_b{B}'] = rec
+        print('ssim_psnr', B, rec, flush=True)
+    opt = get_default_torch_ngp_opt()
+    net = NeRFNetwork(opt)
+    sd = net.state_dict()
+    sd.update(no.make_field_params(seed=0))
+    net.load_state_dict(sd)
+    net = net.cuda().eval()
+    V, hw = 32, 256
+    o, d = zip(*[camera_rays(c, hw, hw) for c in circle_cameras(V, radius=4.5)])
+    rays_o, rays_d = torch.from_numpy(np.stack(o)).cuda(), torch.from_numpy(np.stack(d)).cuda()
+    rgb = torch.rand(V, 3, hw, hw, device='cuda', generator=g)
+    views = ev.EvalViews(rays_o, rays_d, rgb, (rgb > 0.5).float()[:, :1])
+    percep = PerceptualLoss('vgg', device='cuda', seed=1)
+
+    def stamp():
+        e = torch.cuda.Event(enable_timing=True)
+        e.record()
+        return e
+    rows = []
+    with torch.no_grad():
+        for it in range(6):
+            e0 = stamp()
+            imgs = []
+            for v in range(V):
+                with torch.random.fork_rng(devices=[rays_o.device]):
+                    torch.cuda.manual_seed(view_seed(0, 0, v, ev.EVAL_STREAM))
+                    imgs.append(net.render_batched(rays_o[v][None], rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=1.0,
+                                                   shading='albedo', force_all_rays=True, **vars(opt))['image'].reshape(hw, hw, 3))
+            image = torch.stack(imgs)
+            e1 = stamp()
+            lp = [percep.value_and_grad(image[v].permute(2, 0, 1), rgb[v], normalize=True, want_grad=False)[0] for v in range(V)]
+            e2 = stamp()
+            ev.image_metrics(image, rgb.permute(0, 2, 3, 1).contiguous())
+            e3 = stamp()
+            ev.evaluate_scene(net, views, opt, percep, seed=0)
+            e4 = stamp()
+            torch.cuda.synchronize()
+            if it:
+                rows.append((e0.elapsed_time(e1), e1.elapsed_time(e2), e2.elapsed_time(e3), e3.elapsed_time(e4)))
+            del lp
+    med = [float(m) for m in np.median(np.array(rows), axis=0)]
+    rec = dict(views=V, hw=hw, render_ms=round(med[0], 2), lpips_ms=round(med[1], 2), ssim_psnr_ms=round(med[2], 3),
+               evaluate_scene_ms=round(med[3], 2))
+    out['eval']['evaluate_scene_32x256'] = rec
+    print('evaluate_scene', rec, flush=True)
+
+
 def main():
     out = {'device': torch.cuda.get_device_name(0), 'conv': [], 'grid': {}}
+    if 'eval' in sys.argv:
+        eval_bench(out)
+        print(json.dumps(out), flush=True)
+        return
     if 'scenes' in sys.argv:
         scenes_bench(out)
         print(json.dumps(out), flush=True)
