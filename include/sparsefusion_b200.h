@@ -420,6 +420,26 @@ int sfb_marching_cubes_emit(const float* v, int X, int Y, int Z, float iso, cons
 uint64_t sfb_image_ssim_psnr_work(int B, int H, int W);
 int sfb_image_ssim_psnr(const float* a, const float* b, int B, int H, int W, double* out, double* work, void* stream);
 
+/* ==========================================================================================
+ * section 11 -- GIF palettes of the sequence and circle-path gifs (sparsefusion/distillation.py:444-493, which leaves the quantisation to
+ *    imageio / Pillow on the host).  Frames are uint8 [B][H][W][3]; each frame gets its own palette.
+ * ========================================================================================== */
+/* palette [B][256][3] (entries at or beyond ncolors[b] are zero), ncolors [B], indices [B][H][W] of B frames with 2 <= colors <= 256,
+ * a pure function of the input, all integer arithmetic:
+ *   1. histogram: a pixel's cell is (r>>3, g>>3, b>>3) of 32^3; per cell the pixel count n and the sums of the 8-bit r, g, b (uint32).
+ *   2. median cut: a box is an inclusive cell range per axis, always shrunk to the bounding box of its non-empty cells; the first box holds
+ *      every non-empty cell.  While there are fewer than `colors` boxes, the splittable box (some axis with hi > lo) with the largest pixel
+ *      count, lowest index on ties, is split along its axis of largest hi - lo (ties in the order r, g, b) at the smallest t in [lo, hi-1]
+ *      with 2 * (pixels in slices lo..t) >= n (t = hi-1 if there is none).  The lower part keeps the index, the upper part is appended,
+ *      both shrunk.  It stops early when no box is splittable.
+ *   3. palette: entry k = (2 S + N) / (2 N) per channel (box k's channel sum S over its pixel count N, rounded half up); ncolors = boxes.
+ *   4. map: each pixel takes the entry of smallest squared RGB distance, the lowest index on ties.
+ * Three launches (histogram, one CTA per frame for the cut, map).  B in 1..65535, H, W >= 1, H*W <= 16843009 (so that a channel sum fits
+ * 32 bits).  work: sfb_palette_work_bytes(B, H, W) bytes (0 = sizes rejected), zeroed by the call itself. */
+uint64_t sfb_palette_work_bytes(int B, int H, int W);
+int sfb_palette_quantize(const uint8_t* rgb, int B, int H, int W, int colors, uint8_t* palette, int32_t* ncolors, uint8_t* indices, void* work,
+                         void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -75,7 +75,7 @@ def shard_views(views: list, rank: int, world_size: int) -> list:
 
 def view_seed(seed: int, itr: int, view: int, stream: int) -> int:
     """seed of the generator that serves ONE (iteration, view, stream) -- stream 0: photometric render, 1: fusion render, 2: PLMS noise, 3: evaluation
-    render (``evaluate.evaluate_scene``, with iteration 0).
+    render (``evaluate.evaluate_scene``, with iteration 0), 4: circle-path render (``evaluate.render_views`` for the fly-around gif, iteration 0).
     Keyed draws make a minibatch step independent of how its views are spread over ranks."""
     x = (seed * 0x9E3779B97F4A7C15 + itr * 0xBF58476D1CE4E5B9 + view * 0x94D049BB133111EB + stream * 0xD6E8FEB86659FD93) & 0xFFFFFFFFFFFFFFFF
     x ^= x >> 31
@@ -634,33 +634,46 @@ class ReferenceSceneBuilder:
                           target_features=torch.cat(feats) if feats else empty(256, 32, 32), target_eft_image=torch.cat(eft_imgs) if eft_imgs else empty(3, 256, 256),
                           target_rays_o=torch.stack(t_o) if t_o else empty(n_rays, 3), target_rays_d=torch.stack(t_d) if t_d else empty(n_rays, 3))
 
-    def eval_views(self, scene_cameras, scene_rgb, scene_mask):
-        """the views the reference scores the distilled scene on (:393-406): every scene camera in the voxel frame (:70) through the 256x256
-        ``sampler_grid`` (:85), with ``scene_rgb`` / ``scene_mask`` as ground truth -> ``evaluate.EvalViews``"""
+    def _grid_rays(self, scene_cameras, circle_n=None):
+        """rays [V, 256*256, 3] (origins, directions) of the 256x256 ``sampler_grid`` (:85) for every scene camera in the voxel frame (:70,
+        :395-402), or for the ``circle_n`` cameras of the circle path through them (:463-469)"""
         try:
-            from utils.camera_utils import RelativeCameraLoader
+            from utils.camera_utils import RelativeCameraLoader, get_interpolated_path
             from utils.render_utils import init_ray_sampler
         except ImportError as e:
-            raise RuntimeError('distillation_loop(evaluate=True) needs the reference tree (utils/camera_utils.py, utils/render_utils.py) and pytorch3d '
-                               'on sys.path to turn pytorch3d cameras into rays; pass a scene_builder with its own eval_views') from e
+            raise RuntimeError('distillation_loop(evaluate=True / visualize=True) needs the reference tree (utils/camera_utils.py, utils/render_utils.py) '
+                               'and pytorch3d on sys.path to turn pytorch3d cameras into rays; pass a scene_builder with its own eval_views / '
+                               'circle_views') from e
         from einops import rearrange
-        from .evaluate import EvalViews
         relative_cam = RelativeCameraLoader(relative=True, center_at_origin=True)
         relative_cam_no_origin = RelativeCameraLoader(relative=True, center_at_origin=False)
         scene_cameras_vox = relative_cam_no_origin.get_relative_camera(scene_cameras, query_idx=[0], center_at_origin=False)   # :70
         cam_dist_mean = torch.mean(torch.linalg.norm(scene_cameras.get_camera_center(), axis=1))                     # :82-84
         sampler_grid = init_ray_sampler(self.gpu, 256, 256, min=cam_dist_mean - 5.0, max=cam_dist_mean + 5.0, scale_factor=2)[0]   # :85
+        cams = scene_cameras_vox if circle_n is None else get_interpolated_path(scene_cameras_vox, n=circle_n, method='circle')   # :463
         o, d = [], []
-        for ci in range(len(scene_cameras_vox)):                                                                    # :395-402
-            rb = sampler_grid(relative_cam.get_camera_slice(scene_cameras_vox, [ci]))
+        for ci in range(len(cams)):
+            rb = sampler_grid(relative_cam.get_camera_slice(cams, [ci]))
             o.append(rearrange(rb.origins, 'b h w c -> b (h w) c')[0].contiguous())
             d.append(rearrange(rb.directions, 'b h w c -> b (h w) c')[0].contiguous())
-        return EvalViews(rays_o=torch.stack(o), rays_d=torch.stack(d), rgb=scene_rgb.float(), mask=scene_mask.float())
+        return torch.stack(o), torch.stack(d)
+
+    def eval_views(self, scene_cameras, scene_rgb, scene_mask):
+        """the views the reference scores the distilled scene on (:393-406): every scene camera in the voxel frame (:70) through the 256x256
+        ``sampler_grid`` (:85), with ``scene_rgb`` / ``scene_mask`` as ground truth -> ``evaluate.EvalViews``"""
+        from .evaluate import EvalViews
+        o, d = self._grid_rays(scene_cameras)
+        return EvalViews(rays_o=o, rays_d=d, rgb=scene_rgb.float(), mask=scene_mask.float())
+
+    def circle_views(self, scene_cameras, n=50):
+        """the views of the reference's fly-around gif (:461-469): ``get_interpolated_path(scene_cameras_vox, n=50, method='circle')`` through
+        the 256x256 ``sampler_grid`` -> (rays_o, rays_d), each [n, 256*256, 3]"""
+        return self._grid_rays(scene_cameras, circle_n=n)
 
 
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
-                      process_group=None, evaluate=False):
+                      process_group=None, evaluate=False, visualize=False):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -671,11 +684,19 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ``{save_dir}/metrics/{seq_name}.txt`` is written in the reference's format.  LPIPS uses ``loss_fn_vgg``'s weights (an ``lpips.LPIPS``, as
     demo.py:33 passes it, or a ``PerceptualLoss``); without it the LPIPS entry is nan rather than a distance from random VGG weights.
 
-    Not reproduced: the matplotlib loss plots, the periodic / final visualisation renders and gifs (:355-388, :444-493) -- logging, outside the
-    hot path; ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference makes).
+    ``visualize=True`` adds the reference's pictures (:129-141, :444-493; ``_write_scene_pictures``): before the first iteration the builder's
+    ``eval_views`` and ``circle_views(scene_cameras)`` give the scene views and the 50 circle-path views (a builder without them fails then),
+    and with ``use_diffusion`` the grid of cached EFT images is written to ``{args.exp_dir}/log/{seq_name}_eft_grid.jpg``.  After the loop
+    ``{save_dir}/render_gifs/{seq_name}.gif`` (gt | EFT image | render | gt mask | silhouette per scene view, without the EFT panel when not
+    ``use_diffusion``), ``{save_dir}/render_imgs/{seq_name}/{view:03d}.jpg`` (gt | render) and ``{save_dir}/render_gifs/{seq_name}_circle.gif``
+    (render | silhouette per circle view) are written; the sequence frames are the renders ``evaluate`` scores.  GIF palettes are quantised on
+    the GPU (``video.py``); Pillow writes the files.
+
+    Not reproduced: the matplotlib loss plots and the periodic ``_vis.jpg`` renders (:355-388) -- logging, outside the hot path;
+    ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference makes).
     ``scene_valid_region`` is accepted and unused, as in the reference's loop body (:192-195 overwrites the region with ones), and so is
     ``loss_fn_vgg`` unless ``evaluate``.  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
-    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``.
+    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``, ``visualize``.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     rank, world = 0, 1
@@ -687,13 +708,13 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
                          start_percep_step=1000, views_per_step=views_per_step)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
-                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg)
+                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize)
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
-                   evaluate=False, loss_fn_vgg=None):
+                   evaluate=False, loss_fn_vgg=None, visualize=False):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -702,6 +723,7 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     Scenes of one call must share image, latent and ray sizes.  With several GPUs, each rank passes its own share of the scenes.
     ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  ``evaluate`` / ``loss_fn_vgg``: each scene is scored and its
     ``{save_dir}/metrics/{seq_name}.txt`` written as ``distillation_loop(evaluate=True)`` does, scene k's render jitter keyed by ``seed + k``.
+    ``visualize``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter keyed by ``seed + k``.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
 
@@ -710,30 +732,87 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
-                             loss_fn_vgg)
+                             loss_fn_vgg, visualize)
+
+
+EFT_GRID_COLUMNS = 8     # cached EFT images per row of the grid the reference writes before its loop (:129-141)
+
+
+def _write_eft_grid(path, eft_images, n_views):
+    """the reference's ``{exp_dir}/log/{seq_name}_eft_grid.jpg`` (:129-141): the first 8 * ceil(n_views / 8) cached EFT images [N,3,h,w],
+    8 per row"""
+    from .video import to_uint8, write_jpeg
+    rows = -(-n_views // EFT_GRID_COLUMNS)
+    t = eft_images[:rows * EFT_GRID_COLUMNS].float().permute(0, 2, 3, 1)
+    h, w = t.shape[1:3]
+    grid = t.reshape(rows, EFT_GRID_COLUMNS, h, w, 3).permute(0, 2, 1, 3, 4).reshape(1, rows * h, EFT_GRID_COLUMNS * w, 3)
+    write_jpeg(path, to_uint8(grid)[0])
+
+
+def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_images, seed, scores=None):
+    """the reference's sequence gif, per-view jpegs and circle gif of one distilled scene (:444-493).  The sequence frames are ``scores``'
+    renders (``evaluate_scene``'s, the ones the metrics come from) or, without scores, the same renders by ``render_views`` (stream 3);
+    the circle frames are ``render_views`` of the circle rays with stream 4.  ``eft_images``: the scene views' cached EFT images [V,3,h,w]
+    (``use_diffusion``) or None."""
+    from .evaluate import CIRCLE_STREAM, EVAL_STREAM, render_views
+    from .video import to_uint8, write_gif, write_jpegs
+    V = views.rgb.shape[0]
+    H, W = views.rgb.shape[2:]
+    if scores is None:
+        image, sil = render_views(ngp, views.rays_o, views.rays_d, (H, W), opt, seed=seed, stream=EVAL_STREAM)
+    else:
+        image, sil = scores.image, scores.silhouette
+    gt, gt_mask = views.rgb.float().permute(0, 2, 3, 1), views.mask.float().permute(0, 2, 3, 1)
+    eft = [] if eft_images is None else [eft_images[:V].float().permute(0, 2, 3, 1)]
+    gif_path = f'{save_dir}/render_gifs/{seq_name}.gif'
+    write_gif(gif_path, to_uint8(gt, *eft, image, gt_mask, sil[..., None]))                                      # :449-453
+    write_jpegs([f'{save_dir}/render_imgs/{seq_name}/{si:03d}.jpg' for si in range(V)], to_uint8(gt, image))         # :455-456
+    print('saved video', gif_path)
+    rays_o, rays_d = circle
+    hw = int(round(rays_o.shape[1] ** 0.5))
+    if hw * hw != rays_o.shape[1]:
+        raise ValueError(f'circle views must be square images (got {rays_o.shape[1]} rays per view)')
+    c_image, c_sil = render_views(ngp, rays_o, rays_d, (hw, hw), opt, seed=seed, stream=CIRCLE_STREAM)           # :461-485
+    gif_path = f'{save_dir}/render_gifs/{seq_name}_circle.gif'
+    write_gif(gif_path, to_uint8(c_image, c_sil[..., None]))                                                         # :487-490
+    print('saved video', gif_path)
 
 
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
-                      loss_fn_vgg=None):
+                      loss_fn_vgg=None, visualize=False):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
-    ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files (scene k seeded ``seed + k``).
-    Returns the networks."""
+    ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
+    grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``).  Returns the networks."""
     import os
     from .lpips_vgg import PerceptualLoss
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
-    if evaluate and not callable(getattr(builder, 'eval_views', None)):
-        raise TypeError(f'evaluate=True needs the scene builder to provide eval_views(scene_cameras, scene_rgb, scene_mask); '
-                        f'{type(builder).__name__} has none')
+    if visualize:
+        from .video import require_pillow
+        require_pillow()
+    for flag, name, sig in ((evaluate or visualize, 'eval_views', '(scene_cameras, scene_rgb, scene_mask)'), (visualize, 'circle_views', '(scene_cameras)')):
+        if flag and not callable(getattr(builder, name, None)):
+            raise TypeError(f'{"evaluate=True" if name == "eval_views" and evaluate else "visualize=True"} needs the scene builder to provide '
+                            f'{name}{sig}; {type(builder).__name__} has none')
     exp_dir = getattr(args, 'exp_dir', save_dir)
     for sc in scenes:
         os.makedirs(f'{exp_dir}/render_imgs/{sc[0]}/', exist_ok=True)                                                # :57-58
     os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
     os.makedirs(save_dir, exist_ok=True)
     device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
-    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate else None
+    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate or visualize else None
+    circles = [tuple(t.to(device) for t in builder.circle_views(cams)) for _, cams, _, _, _, _ in scenes] if visualize else None
     caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
               for _, cams, rgb, mask, _, input_idx in scenes]
+    if visualize and use_diffusion:
+        for (seq_name, *_rest), views, cache in zip(scenes, eval_views, caches):
+            need = -(-views.rgb.shape[0] // EFT_GRID_COLUMNS) * EFT_GRID_COLUMNS
+            if cache.target_eft_image.shape[0] < need:
+                raise ValueError(f'visualize=True: scene {seq_name} has {views.rgb.shape[0]} views, so its EFT grid needs {need} cached EFT images; '
+                                 f'the cache holds {cache.target_eft_image.shape[0]}')
+        with torch.cuda.device(device):
+            for (seq_name, *_rest), views, cache in zip(scenes, eval_views, caches):
+                _write_eft_grid(f'{exp_dir}/log/{seq_name}_eft_grid.jpg', cache.target_eft_image, views.rgb.shape[0])   # :129-141
     with torch.cuda.device(device):
         perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
         ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
@@ -749,13 +828,18 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
         torch.cuda.synchronize(device)
     for (seq_name, *_rest), ngp in zip(scenes, ngps):
         torch.save({'model_state_dict': ngp.state_dict()}, f'{save_dir}/{seq_name}.pt')                             # :495-496
-    if evaluate:
+    if evaluate or visualize:
         from .evaluate import evaluate_scene, write_scene_metrics
         with torch.cuda.device(device):
-            eval_percep = None if loss_fn_vgg is None else PerceptualLoss('vgg', device=device).load_state_dict(loss_fn_vgg.state_dict())
+            eval_percep = None if loss_fn_vgg is None or not evaluate else PerceptualLoss('vgg', device=device).load_state_dict(loss_fn_vgg.state_dict())
             for k, ((seq_name, *_rest), ngp, views) in enumerate(zip(scenes, ngps, eval_views)):
-                scores = evaluate_scene(ngp, views, opt, eval_percep, seed=base_seed + k)                           # :391-433
-                print('warning: this metric is used for debugging only and not the final metric')
-                print(f'{getattr(args, "category", "")} scene {seq_name}')
-                write_scene_metrics(f'{save_dir}/metrics/{seq_name}.txt', scores)                                  # :434-441
+                scores = None
+                if evaluate:
+                    scores = evaluate_scene(ngp, views, opt, eval_percep, seed=base_seed + k)                       # :391-433
+                    print('warning: this metric is used for debugging only and not the final metric')
+                    print(f'{getattr(args, "category", "")} scene {seq_name}')
+                    write_scene_metrics(f'{save_dir}/metrics/{seq_name}.txt', scores)                              # :434-441
+                if visualize:
+                    _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circles[k], caches[k].target_eft_image if use_diffusion else None,
+                                          base_seed + k, scores)                                                    # :444-493
     return ngps

@@ -18,6 +18,7 @@ from . import _lib as lib
 from .distillation import view_seed
 
 EVAL_STREAM = 3      # view_seed stream of the evaluation renders' jitter
+CIRCLE_STREAM = 4    # view_seed stream of the circle-path renders' jitter (video.py's fly-around gif)
 
 
 @dataclass
@@ -70,12 +71,40 @@ def image_metrics(pred: torch.Tensor, gt: torch.Tensor):
 
 
 @torch.no_grad()
+def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, seed: int, stream: int):
+    """(images [V, H, W, 3] fp32, silhouettes [V, H, W]) of V views (rays [V, H*W, 3], ``hw`` = (H, W)) with the reference's eval-mode render
+    call (distillation.py:404-406, :480-482).  Its ``perturb=True`` jitter, which the reference draws from torch's unseeded global generator,
+    comes from the CUDA generator seeded with ``view_seed(seed, 0, view, stream)`` inside ``torch.random.fork_rng``, so the renders are
+    reproducible and the callers' generators are left as they were.  ``ngp.training`` is restored on return."""
+    dev = rays_o.device
+    if dev.type != 'cuda':
+        raise RuntimeError('render_views: the rays must be CUDA tensors (no CPU fallback)')
+    H, W = hw
+    V, N = rays_o.shape[:2]
+    if N != H * W or rays_d.shape != rays_o.shape:
+        raise ValueError(f'render_views: rays {tuple(rays_o.shape)} / {tuple(rays_d.shape)} do not match {H} x {W} images')
+    was_training = ngp.training
+    ngp.eval()
+    images, sils = [], []
+    try:
+        with torch.cuda.device(dev):
+            for v in range(V):
+                with torch.random.fork_rng(devices=[dev]):
+                    torch.cuda.manual_seed(view_seed(seed, 0, v, stream))
+                    out = ngp.render_batched(rays_o[v][None], rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=1.0,
+                                             shading='albedo', force_all_rays=True, **vars(opt))
+                images.append(out['image'].reshape(H, W, 3))
+                sils.append(out['weights_sum'].reshape(H, W))
+            return torch.stack(images).float(), torch.stack(sils)
+    finally:
+        ngp.train(was_training)
+
+
+@torch.no_grad()
 def evaluate_scene(ngp, views: EvalViews, opt, percep, *, seed: int) -> SceneEval:
-    """scores of ``ngp`` on every view of ``views`` (distillation.py:393-433).  Each view gets the reference's render call (:404-406) in eval mode;
-    its ``perturb=True`` jitter, which the reference draws from torch's unseeded global generator, comes from the CUDA generator seeded with
-    ``view_seed(seed, 0, view, 3)`` inside ``torch.random.fork_rng``, so a score is reproducible and the callers' generators are left as they
-    were.  SSIM / PSNR: ``image_metrics`` over all views at once.  LPIPS: ``percep.value_and_grad(render, gt, normalize=True, want_grad=False)``
-    per view, which is the reference's ``loss_fn_vgg(gt * 2 - 1, pred * 2 - 1)`` (the distance is symmetric); nan when ``percep`` is None.
+    """scores of ``ngp`` on every view of ``views`` (distillation.py:393-433).  The renders are ``render_views`` with ``stream=3``: the
+    reference's eval-mode render call, jitter from ``view_seed(seed, 0, view, 3)``, the callers' generators left as they were.  SSIM / PSNR:
+    ``image_metrics`` over all views at once.  LPIPS: ``percep.value_and_grad(render, gt, normalize=True, want_grad=False)`` per view, which is the reference's ``loss_fn_vgg(gt * 2 - 1, pred * 2 - 1)`` (the distance is symmetric); nan when ``percep`` is None.
     ``ngp.training`` is restored on return."""
     dev = views.rays_o.device
     if dev.type != 'cuda':
@@ -84,28 +113,15 @@ def evaluate_scene(ngp, views: EvalViews, opt, percep, *, seed: int) -> SceneEva
     H, W = views.rgb.shape[2:]
     if N != H * W or views.rgb.shape[:2] != (V, 3) or views.rays_d.shape != views.rays_o.shape:
         raise ValueError(f'evaluate_scene: rays {tuple(views.rays_o.shape)} / {tuple(views.rays_d.shape)} do not match images {tuple(views.rgb.shape)}')
-    was_training = ngp.training
-    ngp.eval()
-    images, sils = [], []
-    try:
-        with torch.cuda.device(dev):
-            for v in range(V):
-                with torch.random.fork_rng(devices=[dev]):
-                    torch.cuda.manual_seed(view_seed(seed, 0, v, EVAL_STREAM))
-                    out = ngp.render_batched(views.rays_o[v][None], views.rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=1.0,
-                                             shading='albedo', force_all_rays=True, **vars(opt))
-                images.append(out['image'].reshape(H, W, 3))
-                sils.append(out['weights_sum'].reshape(H, W))
-            image, sil = torch.stack(images).float(), torch.stack(sils)
-            gt = views.rgb.float().permute(0, 2, 3, 1).contiguous()
-            ssim, psnr = image_metrics(image, gt)
-            if percep is None:
-                lp = torch.full((V,), float('nan'), dtype=torch.float64, device=dev)
-            else:
-                lp = torch.stack([percep.value_and_grad(image[v].permute(2, 0, 1), views.rgb[v].float(), normalize=True, want_grad=False)[0]
-                                  for v in range(V)]).double()
-    finally:
-        ngp.train(was_training)
+    image, sil = render_views(ngp, views.rays_o, views.rays_d, (H, W), opt, seed=seed, stream=EVAL_STREAM)
+    with torch.cuda.device(dev):
+        gt = views.rgb.float().permute(0, 2, 3, 1).contiguous()
+        ssim, psnr = image_metrics(image, gt)
+        if percep is None:
+            lp = torch.full((V,), float('nan'), dtype=torch.float64, device=dev)
+        else:
+            lp = torch.stack([percep.value_and_grad(image[v].permute(2, 0, 1), views.rgb[v].float(), normalize=True, want_grad=False)[0]
+                              for v in range(V)]).double()
     return SceneEval(psnr=psnr, ssim=ssim, lpips=lp, image=image, silhouette=sil)
 
 

@@ -547,8 +547,92 @@ def eval_bench(out):
     print('evaluate_scene', rec, flush=True)
 
 
+def video_bench(out):
+    """gif palettes (sparsefusion_b200.video): sfb_palette_quantize on render-like frames (black background, a textured blob per panel) --
+    50 frames of 256x512 (the circle gif) and V = 32 / 200 frames of 256x1280 (the sequence gif) -- by CUDA events around 10 calls after a
+    warm-up; Pillow's convert('P', palette=ADAPTIVE) on the same frames by a host clock; and the end-to-end visualize step of one scene
+    (_write_scene_pictures: 32 views and 50 circle views at 256^2 rendered, quantised and written) by a host clock around a synchronise."""
+    import subprocess
+    import tempfile
+    import time
+    from PIL import Image
+    from oracle import ngp_oracle as no
+    from sparsefusion_b200 import evaluate as ev, video
+    from sparsefusion_b200.distillation import _write_scene_pictures
+    from sparsefusion_b200.network_grid import NeRFNetwork, get_default_torch_ngp_opt
+    from sparsefusion_b200.synthetic import camera_rays, circle_cameras
+    out['card'] = subprocess.run(['nvidia-smi', '--query-gpu=name,power.limit,clocks.max.sm', '--format=csv,noheader'], capture_output=True,
+                                 text=True).stdout.strip()
+    print('card', out['card'], flush=True)
+    out['video'] = {}
+    g = torch.Generator(device='cuda').manual_seed(0)
+
+    def render_like(B, H, W):
+        yy, xx = torch.meshgrid(torch.arange(H, device='cuda'), torch.arange(W // 256 * 256, device='cuda') % 256, indexing='ij')
+        c = torch.rand(B, 1, 1, 2, device='cuda', generator=g) * 80 + 88
+        blob = (1 - ((yy - c[..., 0]) ** 2 + (xx - c[..., 1]) ** 2) / 70.0 ** 2).clamp(0, 1)
+        return video.to_uint8(blob[..., None] * (0.5 + 0.5 * torch.rand(B, H, W, 3, device='cuda', generator=g)))
+
+    for name, (B, H, W) in (('circle_50x256x512', (50, 256, 512)), ('sequence_32x256x1280', (32, 256, 1280)), ('sequence_200x256x1280', (200, 256, 1280))):
+        frames = render_like(B, H, W)
+        for _ in range(3):
+            video.quantize_palette(frames)
+        torch.cuda.synchronize()
+        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        t0.record()
+        for _ in range(10):
+            video.quantize_palette(frames)
+        t1.record()
+        torch.cuda.synchronize()
+        ms = t0.elapsed_time(t1) / 10
+        host = frames.cpu().numpy()
+        h0 = time.perf_counter()
+        for f in host:
+            Image.fromarray(f).convert('P', palette=Image.ADAPTIVE)
+        pil_ms = (time.perf_counter() - h0) * 1e3
+        rec = dict(gpu_ms=round(ms, 3), gpu_us_per_frame=round(ms * 1e3 / B, 1), pillow_ms=round(pil_ms, 1), pillow_ms_per_frame=round(pil_ms / B, 1),
+                   ncolors_mean=round(video.quantize_palette(frames)[1].float().mean().item(), 1))
+        out['video'][name] = rec
+        print('quantize', name, rec, flush=True)
+    opt = get_default_torch_ngp_opt()
+    net = NeRFNetwork(opt)
+    sd = net.state_dict()
+    sd.update(no.make_field_params(seed=0))
+    net.load_state_dict(sd)
+    net = net.cuda().eval()
+    V, hw = 32, 256
+    o, d = zip(*[camera_rays(c, hw, hw) for c in circle_cameras(V, radius=4.5)])
+    rgb = torch.rand(V, 3, hw, hw, device='cuda', generator=g)
+    views = ev.EvalViews(torch.from_numpy(np.stack(o)).cuda(), torch.from_numpy(np.stack(d)).cuda(), rgb, (rgb > 0.5).float()[:, :1])
+    co, cd = zip(*[camera_rays(c, hw, hw) for c in circle_cameras(50, radius=4.0)])
+    circle = torch.from_numpy(np.stack(co)).cuda(), torch.from_numpy(np.stack(cd)).cuda()
+    eft = torch.rand(V, 3, hw, hw, device='cuda', generator=g)
+    times, renders = [], []
+    with tempfile.TemporaryDirectory() as tmp:
+        for it in range(4):
+            torch.cuda.synchronize()
+            h0 = time.perf_counter()
+            _write_scene_pictures(tmp, 'scene', net, opt, views, circle, eft, seed=0)
+            torch.cuda.synchronize()
+            h1 = time.perf_counter()
+            ev.render_views(net, views.rays_o, views.rays_d, (hw, hw), opt, seed=0, stream=ev.EVAL_STREAM)     # the same renders alone
+            ev.render_views(net, *circle, (hw, hw), opt, seed=0, stream=ev.CIRCLE_STREAM)
+            torch.cuda.synchronize()
+            if it:
+                times.append((h1 - h0) * 1e3)
+                renders.append((time.perf_counter() - h1) * 1e3)
+    rec = dict(views=V, circle_views=50, hw=hw, visualize_ms=round(float(np.median(times)), 1), renders_ms=round(float(np.median(renders)), 1),
+               all_ms=[round(t, 1) for t in times])
+    out['video']['visualize_one_scene'] = rec
+    print('visualize', rec, flush=True)
+
+
 def main():
     out = {'device': torch.cuda.get_device_name(0), 'conv': [], 'grid': {}}
+    if 'video' in sys.argv:
+        video_bench(out)
+        print(json.dumps(out), flush=True)
+        return
     if 'eval' in sys.argv:
         eval_bench(out)
         print(json.dumps(out), flush=True)
