@@ -282,6 +282,29 @@ int sfb_ngp_field_backward(const float* xyz, const float* rays_o, const float* r
                            float* gb2, float* tape, void* stream);
 uint32_t sfb_ngp_field_tape_points(uint32_t B);
 uint64_t sfb_ngp_field_tape_floats(uint32_t B);
+/* Finite-difference normals of the field (network_grid.py:91-164) as stencils on the tiled field kernel: the stencil rows
+ * (point, slot, jitter sample) are generated and reduced inside the kernel, so no 6B or 60B point array exists in memory.
+ *   slots = 6: slot s shifts component s/2 by +eps (even s) or -eps (odd s) and clamps to [-bound, bound]; each slot is the mean
+ *              of k samples.  fd [B,3] = 0.5 (sigma+ - sigma-) / eps and normal [B,3] = safe_normalize(fd), NaN -> 0 (either
+ *              may be NULL).  k = 1 without a key: finite_difference_normal(x, eps); k = 10, eps = radius = 0.3:
+ *              finite_difference_normal_smooth.
+ *   slots = 1: common_forward_smooth(x, radius, k): sigma [B] and albedo [B,3] (or NULL), the means over k samples.
+ * A sample adds the jitter (u radius) 2 - radius, not clamped, with u from Philox4x32-10 (counter (point, slot, sample, 0),
+ * key = *key as two 32-bit words, low first; u = (r >> 8) 2^-24 of lanes 0..2); the blob is evaluated at the un-jittered point.
+ * key is device memory (NULL: no jitter; required when k > 1).  slots * k <= 128.  Always the tiled kernels. */
+int sfb_ngp_field_normal_forward(const float* xyz, const float* rays_o, const float* rays_d, const float* z, uint32_t T, uint32_t B,
+                                 const float* embeddings, const int32_t* offsets, float S, uint32_t H, float bound, const float* W0,
+                                 const float* b0, const float* W1, const float* b1, const float* W2, const float* b2, uint32_t slots,
+                                 uint32_t k, float eps, float radius, const int64_t* key, float* fd, float* normal, float* sigma,
+                                 float* albedo, void* stream);
+/* Backward of the plain stencil (slots = 6, k = 1) w.r.t. every parameter, ACCUMULATED into caller-zeroed buffers like
+ * sfb_ngp_field_backward.  Give grad_fd [B,3] (dL/dfd), or grad_normal [B,3] with the forward's fd [B,3]: the safe_normalize
+ * backward, zero in components whose normal was NaN and for points whose fd is not finite. */
+int sfb_ngp_field_normal_backward(const float* xyz, const float* rays_o, const float* rays_d, const float* z, uint32_t T, uint32_t B,
+                                  const float* embeddings, const int32_t* offsets, float S, uint32_t H, float bound, const float* W0,
+                                  const float* b0, const float* W1, const float* b1, const float* W2, const float* b2, float eps,
+                                  const float* fd, const float* grad_normal, const float* grad_fd, float* grad_embeddings, float* gW0,
+                                  float* gb0, float* gW1, float* gb1, float* gW2, float* gb2, void* stream);
 /* The per-ray stages of NeRFRenderer.run (external/nerf/renderer_df.py:310-468; num_steps = upsample_steps = 64), one warp per ray.
  * All random draws of the reference are inputs: noise [N,64] U(0,1) or NULL (perturb=False, :363); u [N,64] (torch.rand at :31, or the
  * deterministic linspace of :28 in eval mode).  lin = torch.linspace(0,1,64) (:356), passed in so depths are bit-identical to torch's. */

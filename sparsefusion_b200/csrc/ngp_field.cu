@@ -799,11 +799,31 @@ __device__ __forceinline__ void encode_levels_p64(const float (&x)[3], bool vali
     }
 }
 
-__global__ void __launch_bounds__(kBT, 2) field_backward_v2_kernel(PointSource ps, uint32_t B, const float* __restrict__ table, const int32_t* __restrict__ offsets,
+// The rows the tiled backward walks.  PointRows: one row per field point, upstream gradients dL/dsigma [B] and dL/drgb [B,3] (or NULL).
+// (StencilRows, below with the normal kernels, generates the six finite-difference rows of each point instead.)
+struct PointRows {
+    PointSource ps;
+    uint32_t B;
+    const float* g_sigma;
+    const float* g_rgb;
+    __device__ __forceinline__ uint32_t tiles() const { return (B + kPB - 1) / kPB; }
+    // row `pt` of backward tile `tile`: its point x and row index r; false for padding rows
+    __device__ __forceinline__ bool fetch(uint32_t tile, int pt, float (&x)[3], uint32_t& r) const {
+        r = tile * kPB + pt;
+        if (r >= B) return false;
+        fetch_point(ps, r, x);
+        return true;
+    }
+    __device__ __forceinline__ float grad_sigma(uint32_t r) const { return g_sigma[r]; }
+    __device__ __forceinline__ bool has_rgb() const { return g_rgb != nullptr; }
+    __device__ __forceinline__ float grad_rgb(uint32_t r, int c) const { return g_rgb[(size_t)r * 3 + c]; }
+};
+
+template <class Rows>
+__global__ void __launch_bounds__(kBT, 2) field_backward_v2_kernel(Rows rows, const float* __restrict__ table, const int32_t* __restrict__ offsets,
                                                                   FieldGeom g, const float* __restrict__ W0, const float* __restrict__ b0,
                                                                   const float* __restrict__ W1, const float* __restrict__ b1, const float* __restrict__ W2,
-                                                                  const float* __restrict__ b2, const float* __restrict__ g_sigma,
-                                                                  const float* __restrict__ g_rgb, float* __restrict__ grad_table, float* __restrict__ gW0,
+                                                                  const float* __restrict__ b2, float* __restrict__ grad_table, float* __restrict__ gW0,
                                                                   float* __restrict__ gb0, float* __restrict__ gW1, float* __restrict__ gb1,
                                                                   float* __restrict__ gW2, float* __restrict__ gb2) {
     extern __shared__ __align__(16) uint8_t smraw[];
@@ -829,12 +849,11 @@ __global__ void __launch_bounds__(kBT, 2) field_backward_v2_kernel(PointSource p
     float aW2[2] = {0.f, 0.f};      // dW2[c][k]: k = tid & 63, c = (tid >> 6) + 2 i
     float ab1 = 0.f;                // tid < 64: db1[tid]; tid >= 64: db0[tid - 64]
     float ab2 = 0.f;                // tid < 4: db2[tid]
-    const uint32_t tiles = (B + kPB - 1) / kPB;
+    const uint32_t tiles = rows.tiles();
     for (uint32_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
-        const uint32_t p = tile * kPB + pt;
-        const bool valid = p < B;
+        uint32_t p;
         float x[3] = {0.f, 0.f, 0.f};
-        if (valid) fetch_point(ps, p, x);
+        const bool valid = rows.fetch(tile, pt, x, p);
         // ---- forward recompute: E -> H1 -> H2
         encode_levels_p64(x, valid, table, offsets, g, bufA, pt, half * 8, 8);
         __syncthreads();
@@ -854,11 +873,11 @@ __global__ void __launch_bounds__(kBT, 2) field_backward_v2_kernel(PointSource p
                     o[0] += w.x * hk; o[1] += w.y * hk; o[2] += w.z * hk; o[3] += w.w * hk;
                 }
                 const float pre = o[0] + density_blob(x);
-                d3[0] = g_sigma[p] * expf(fminf(fmaxf(pre, -15.f), 15.f));       // trunc_exp backward (ngp_activation.py:19-21)
+                d3[0] = rows.grad_sigma(p) * expf(fminf(fmaxf(pre, -15.f), 15.f));       // trunc_exp backward (ngp_activation.py:19-21)
 #pragma unroll
                 for (int c = 0; c < 3; ++c) {
                     const float sg = 1.f / (1.f + expf(-o[c + 1]));
-                    d3[c + 1] = g_rgb ? g_rgb[(size_t)p * 3 + c] * sg * (1.f - sg) : 0.f;
+                    d3[c + 1] = rows.has_rgb() ? rows.grad_rgb(p, c) * sg * (1.f - sg) : 0.f;
                 }
             }
 #pragma unroll
@@ -957,6 +976,206 @@ __global__ void __launch_bounds__(kBT, 2) field_backward_v2_kernel(PointSource p
     }
 }
 
+// ================================================================================================ finite-difference normals
+// NeRFNetwork.finite_difference_normal / _smooth / common_forward_smooth / normal (external/nerf/network_grid.py:91-164) as stencils on
+// the tiled field kernels.  The rows of a tile are (point, slot, sample): slot s in 0..5 shifts component s / 2 by +eps (even s) or -eps
+// (odd s) and clamps to [-bound, bound] (:93-98, :139-144); sample j adds the jitter (u radius) 2 - radius with no clamp after it
+// (:112-114).  The blob is evaluated at the un-jittered (shifted, clamped) point (:123).  Only output row 0 (and, for the centre-only
+// stencil, rows 1..3) of the last layer is computed, and a segmented reduction in shared memory turns each point's rows into
+// fd [B,3] = 0.5 (mean sigma+ - mean sigma-) / eps and normal = safe_normalize(fd) with NaN -> 0 (:155-164, utils.py:41-42).
+//
+// Jitter: Philox4x32-10 (Salmon et al., SC'11; the Random123 constants), counter (point, slot, sample, 0), key = the 64-bit value at
+// `key` (low word first).  Lanes 0..2 give the three components' uniforms u = (r >> 8) 2^-24.
+__device__ __forceinline__ uint4 philox4x32_10(uint4 c, uint2 k) {
+#pragma unroll
+    for (int i = 0; i < 10; ++i) {
+        const uint32_t lo0 = 0xD2511F53u * c.x, hi0 = __umulhi(0xD2511F53u, c.x);
+        const uint32_t lo1 = 0xCD9E8D57u * c.z, hi1 = __umulhi(0xCD9E8D57u, c.z);
+        c = make_uint4(hi1 ^ c.y ^ k.x, lo1, hi0 ^ c.w ^ k.y, lo0);
+        k.x += 0x9E3779B9u;
+        k.y += 0xBB67AE85u;
+    }
+    return c;
+}
+
+// x + eps e_{slot/2} (even slot) or x - eps e_{slot/2} (odd slot), clamped to [-bound, bound]; no register-indexed arrays
+__device__ __forceinline__ void shift_clamp(float (&x)[3], uint32_t slot, float eps, float bound) {
+    const float e = (slot & 1) ? -eps : eps;
+#pragma unroll
+    for (uint32_t d = 0; d < 3; ++d) {
+        const float v = d == (slot >> 1) ? __fadd_rn(x[d], e) : x[d];
+        x[d] = fminf(fmaxf(v, -bound), bound);
+    }
+}
+
+struct StencilSpec {
+    uint32_t slots;     // 6: the finite-difference stencil; 1: the centre only (common_forward_smooth)
+    uint32_t k;         // jitter samples per slot (1 and no key: the plain stencil)
+    uint32_t R;         // rows per point = slots * k (<= kPT)
+    uint32_t ppt;       // points per 128-row tile = kPT / R
+    float eps, radius, bound;
+    const int64_t* key; // device-resident Philox key, or NULL: no jitter
+};
+
+// the stencil point of row (q, slot, sample): x is what the grid sees, xb where the blob is evaluated
+__device__ __forceinline__ void stencil_point(const PointSource& ps, const StencilSpec& st, uint2 key, uint32_t q, uint32_t slot, uint32_t smp,
+                                              float (&x)[3], float (&xb)[3]) {
+    fetch_point(ps, q, x);
+    if (st.slots == 6) shift_clamp(x, slot, st.eps, st.bound);
+#pragma unroll
+    for (int d = 0; d < 3; ++d) xb[d] = x[d];
+    if (st.key) {
+        const uint4 r = philox4x32_10(make_uint4(q, slot, smp, 0u), key);
+        const uint32_t rr[3] = {r.x, r.y, r.z};
+#pragma unroll
+        for (int d = 0; d < 3; ++d) {
+            const float u = __uint2float_rn(rr[d] >> 8) * 0x1p-24f;
+            x[d] = __fadd_rn(x[d], __fsub_rn(__fmul_rn(__fmul_rn(u, st.radius), 2.f), st.radius));    // x + (rand * radius * 2 - radius)
+        }
+    }
+}
+
+__device__ __forceinline__ uint2 load_key(const int64_t* key) {
+    if (!key) return make_uint2(0u, 0u);
+    const uint64_t k = (uint64_t)*key;
+    return make_uint2((uint32_t)k, (uint32_t)(k >> 32));
+}
+
+// safe_normalize(fd) (utils.py:41-42: the clamp is on the squared norm) with NaN -> 0 (network_grid.py:161-162)
+__device__ __forceinline__ void safe_normalize_nan0(const float (&fd)[3], float (&n)[3]) {
+    const float r = sqrtf(fmaxf(fd[0] * fd[0] + fd[1] * fd[1] + fd[2] * fd[2], 1e-20f));
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+        const float v = fd[a] / r;
+        n[a] = isnan(v) ? 0.f : v;
+    }
+}
+
+__global__ void __launch_bounds__(kPT) field_stencil_forward_kernel(PointSource ps, uint32_t B, StencilSpec st, const float* __restrict__ table,
+                                                                   const int32_t* __restrict__ offsets, FieldGeom g, const float* __restrict__ W0,
+                                                                   const float* __restrict__ b0, const float* __restrict__ W1, const float* __restrict__ b1,
+                                                                   const float* __restrict__ W2, const float* __restrict__ b2, float* __restrict__ fd_out,
+                                                                   float* __restrict__ normal_out, float* __restrict__ sigma_out,
+                                                                   float* __restrict__ albedo_out) {
+    extern __shared__ __align__(16) uint8_t smraw[];
+    FieldSmemV2& s = *reinterpret_cast<FieldSmemV2*>(smraw);
+    float* bufA = reinterpret_cast<float*>(smraw + sizeof(FieldSmemV2));      // E (rows 0..31), then H2
+    float* bufB = bufA + kHid * kLd;                                         // H1, then the rows' sigma (row 0) and albedo (rows 1..3)
+    load_weights_v2(s, W0, b0, W1, b1, W2, b2);
+    const uint2 key = load_key(st.key);
+    __syncthreads();
+    const int tid = threadIdx.x;
+    const bool centre = st.slots == 1;
+    const uint32_t lp = tid / st.R, rr = tid - lp * st.R, slot = rr / st.k, smp = rr - slot * st.k;
+    const uint32_t tiles = (B + st.ppt - 1) / st.ppt;
+    for (uint32_t tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+        const uint32_t q = tile * st.ppt + lp;
+        const bool valid = lp < st.ppt && q < B;
+        float x[3] = {0.f, 0.f, 0.f}, xb[3] = {0.f, 0.f, 0.f};
+        if (valid) stencil_point(ps, st, key, q, slot, smp, x, xb);
+        encode_point_tile(x, valid, table, offsets, g, bufA, tid);
+        __syncthreads();
+        dense_tile64<kIn, 0>(s.WT0, s.b0, bufA, bufB, nullptr);
+        __syncthreads();
+        dense_tile64<kHid, 0>(s.WT1, s.b1, bufB, bufA, nullptr);
+        __syncthreads();
+        if (valid) {
+            float o0 = s.b2[0], o1 = s.b2[1], o2 = s.b2[2], o3 = s.b2[3];
+#pragma unroll 8
+            for (int k = 0; k < kHid; ++k) {
+                const float hk = bufA[k * kLd + tid];
+                const float4 w = *reinterpret_cast<const float4*>(s.WT2 + k * kOut);
+                o0 += w.x * hk;
+                if (centre) { o1 += w.y * hk; o2 += w.z * hk; o3 += w.w * hk; }
+            }
+            bufB[tid] = expf(o0 + density_blob(xb));
+            if (centre) {
+                bufB[kLd + tid] = 1.f / (1.f + expf(-o1));
+                bufB[2 * kLd + tid] = 1.f / (1.f + expf(-o2));
+                bufB[3 * kLd + tid] = 1.f / (1.f + expf(-o3));
+            }
+        }
+        __syncthreads();
+        // segmented reduction: one thread per point over its R rows (slot-major, samples in order, then / k as torch's mean does)
+        const uint32_t qo = tile * st.ppt + tid;
+        if ((uint32_t)tid < st.ppt && qo < B) {
+            const float* row = bufB + tid * st.R;
+            const float kf = (float)st.k;
+            if (centre) {
+#pragma unroll 1
+                for (int c = 0; c < 4; ++c) {
+                    float t = 0.f;
+                    for (uint32_t j = 0; j < st.k; ++j) t += row[c * kLd + j];
+                    if (c == 0) sigma_out[qo] = t / kf;
+                    else if (albedo_out) albedo_out[(size_t)qo * 3 + c - 1] = t / kf;
+                }
+            } else {
+                float m[6];
+#pragma unroll
+                for (int sl = 0; sl < 6; ++sl) {
+                    float t = 0.f;
+                    for (uint32_t j = 0; j < st.k; ++j) t += row[sl * st.k + j];
+                    m[sl] = t / kf;
+                }
+                float fd[3], n[3];
+#pragma unroll
+                for (int a = 0; a < 3; ++a) fd[a] = __fdiv_rn(__fmul_rn(0.5f, __fsub_rn(m[2 * a], m[2 * a + 1])), st.eps);   // 0.5 * (pos - neg) / eps
+                safe_normalize_nan0(fd, n);
+#pragma unroll
+                for (int a = 0; a < 3; ++a) {
+                    if (fd_out) fd_out[(size_t)qo * 3 + a] = fd[a];
+                    if (normal_out) normal_out[(size_t)qo * 3 + a] = n[a];
+                }
+            }
+        }
+        __syncthreads();     // bufA / bufB are rewritten by the next tile
+    }
+}
+
+// Backward rows of the plain stencil (no jitter): 10 points x 6 slots = 60 of a 64-row backward tile.  dL/dsigma of slot s of point q is
+// +-0.5 g_fd / eps, with g_fd = grad_fd [B,3] directly, or the safe_normalize backward of grad_normal [B,3] at fd [B,3]: zero in the
+// components whose normal was NaN (network_grid.py:162 writes 0 there), and zero for a point whose fd is not finite.
+constexpr int kStencilPB = kPB / 6;
+struct StencilRows {
+    PointSource ps;
+    uint32_t B;
+    float eps, bound;
+    const float* fd;
+    const float* g_normal;
+    const float* g_fd;
+    __host__ __device__ __forceinline__ uint32_t tiles() const { return (B + kStencilPB - 1) / kStencilPB; }
+    __device__ __forceinline__ bool fetch(uint32_t tile, int pt, float (&x)[3], uint32_t& r) const {
+        const uint32_t q = tile * kStencilPB + pt / 6, slot = pt % 6;
+        if (pt >= kStencilPB * 6 || q >= B) return false;
+        r = q * 6 + slot;
+        fetch_point(ps, q, x);
+        shift_clamp(x, slot, eps, bound);
+        return true;
+    }
+    __device__ __forceinline__ float grad_sigma(uint32_t r) const {
+        const uint32_t q = r / 6, slot = r - q * 6, a = slot >> 1;
+        float gfd;
+        if (g_fd) {
+            gfd = g_fd[(size_t)q * 3 + a];
+        } else {
+            const float f0 = fd[(size_t)q * 3], f1 = fd[(size_t)q * 3 + 1], f2 = fd[(size_t)q * 3 + 2];
+            const float ss = f0 * f0 + f1 * f1 + f2 * f2;
+            if (!isfinite(ss)) return 0.f;
+            const float rn = sqrtf(fmaxf(ss, 1e-20f));
+            // dL/dfd = (g - n (n . g)) / r over the components that were not NaN (none is, once ss is finite)
+            const float g0 = g_normal[(size_t)q * 3], g1 = g_normal[(size_t)q * 3 + 1], g2 = g_normal[(size_t)q * 3 + 2];
+            const float dot = g0 * f0 + g1 * f1 + g2 * f2;
+            const float fa = a == 0 ? f0 : (a == 1 ? f1 : f2), ga = a == 0 ? g0 : (a == 1 ? g1 : g2);
+            gfd = ga / rn;
+            if (ss > 1e-20f) gfd -= fa * (dot / (rn * rn * rn));
+        }
+        const float gd = 0.5f * (gfd / eps);
+        return (slot & 1) ? -gd : gd;
+    }
+    __device__ __forceinline__ bool has_rgb() const { return false; }
+    __device__ __forceinline__ float grad_rgb(uint32_t, int) const { return 0.f; }
+};
+
 static int field_args_ok(const float* table, const int32_t* offsets, const float* W0, const float* b0, const float* W1, const float* b1,
                          const float* W2, const float* b2) {
     return table && offsets && W0 && b0 && W1 && b1 && W2 && b2;
@@ -1015,11 +1234,11 @@ int sfb_ngp_field_backward(const float* xyz, const float* rays_o, const float* r
     if (field_v2_enabled()) {
         // tiled kernel: activations stay in shared memory, weight gradients accumulate in registers per CTA -- `tape` is not touched
         const size_t smem2 = sizeof(FieldSmemV2Bwd) + (size_t)(kIn + 2 * kHid) * kLdB * 4;
-        SFB_ONCE_PER_DEVICE(SFB_CUDA(cudaFuncSetAttribute(field_backward_v2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2)));
+        SFB_ONCE_PER_DEVICE(SFB_CUDA(cudaFuncSetAttribute(field_backward_v2_kernel<PointRows>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2)));
         const uint32_t tiles = ceil_div(B, (uint32_t)kPB);
         const uint32_t blocks2 = min(tiles, (uint32_t)sm_count() * 2);
-        field_backward_v2_kernel<<<blocks2, kBT, smem2, as_stream(stream)>>>(make_source(xyz, rays_o, rays_d, z, T, bound), B, embeddings, offsets,
-                                                                            FieldGeom{S, H, bound}, W0, b0, W1, b1, W2, b2, grad_sigma, grad_rgb,
+        const PointRows rows{make_source(xyz, rays_o, rays_d, z, T, bound), B, grad_sigma, grad_rgb};
+        field_backward_v2_kernel<<<blocks2, kBT, smem2, as_stream(stream)>>>(rows, embeddings, offsets, FieldGeom{S, H, bound}, W0, b0, W1, b1, W2, b2,
                                                                             grad_embeddings, gW0, gb0, gW1, gb1, gW2, gb2);
         return check_launch("ngp_field_backward(v2)");
     }
@@ -1060,6 +1279,44 @@ int sfb_ngp_field_backward(const float* xyz, const float* rays_o, const float* r
     mlp_wgrad_kernel<kOut, kHid><<<wb, 256, 0, st>>>(D3, H2, Bp, gW2, gb2);
     count_launches(2);
     return check_launch("ngp_field_backward(weights)");
+}
+
+int sfb_ngp_field_normal_forward(const float* xyz, const float* rays_o, const float* rays_d, const float* z, uint32_t T, uint32_t B,
+                                 const float* embeddings, const int32_t* offsets, float S, uint32_t H, float bound, const float* W0, const float* b0,
+                                 const float* W1, const float* b1, const float* W2, const float* b2, uint32_t slots, uint32_t k, float eps,
+                                 float radius, const int64_t* key, float* fd, float* normal, float* sigma, float* albedo, void* stream) {
+    if (B == 0) return SFB_OK;
+    SFB_REQUIRE(field_args_ok(embeddings, offsets, W0, b0, W1, b1, W2, b2), "ngp_field_normal_forward: null pointer");
+    SFB_REQUIRE(xyz || (rays_o && rays_d && z && T > 0), "ngp_field_normal_forward: give xyz or (rays_o, rays_d, z, T)");
+    SFB_REQUIRE((slots == 6 && (fd || normal) && eps != 0.f) || (slots == 1 && sigma), "ngp_field_normal_forward: slots must be 6 (fd / normal) or 1 (sigma)");
+    SFB_REQUIRE(k >= 1 && slots * k <= (uint32_t)kPT && (k == 1 || key), "ngp_field_normal_forward: need 1 <= slots * k <= 128, and a key when k > 1");
+    const StencilSpec st{slots, k, slots * k, kPT / (slots * k), eps, radius, bound, key};
+    const size_t smem = sizeof(FieldSmemV2) + (size_t)2 * kHid * kLd * 4;
+    SFB_ONCE_PER_DEVICE(SFB_CUDA(cudaFuncSetAttribute(field_stencil_forward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
+    const uint32_t blocks = min(ceil_div(B, st.ppt), (uint32_t)sm_count() * 2);
+    field_stencil_forward_kernel<<<blocks, kPT, smem, as_stream(stream)>>>(make_source(xyz, rays_o, rays_d, z, T, bound), B, st, embeddings, offsets,
+                                                                          FieldGeom{S, H, bound}, W0, b0, W1, b1, W2, b2, fd, normal, sigma, albedo);
+    return check_launch("ngp_field_normal_forward");
+}
+
+int sfb_ngp_field_normal_backward(const float* xyz, const float* rays_o, const float* rays_d, const float* z, uint32_t T, uint32_t B,
+                                  const float* embeddings, const int32_t* offsets, float S, uint32_t H, float bound, const float* W0, const float* b0,
+                                  const float* W1, const float* b1, const float* W2, const float* b2, float eps, const float* fd,
+                                  const float* grad_normal, const float* grad_fd, float* grad_embeddings, float* gW0, float* gb0, float* gW1,
+                                  float* gb1, float* gW2, float* gb2, void* stream) {
+    if (B == 0) return SFB_OK;
+    SFB_REQUIRE(field_args_ok(embeddings, offsets, W0, b0, W1, b1, W2, b2) && grad_embeddings && gW0 && gb0 && gW1 && gb1 && gW2 && gb2,
+                "ngp_field_normal_backward: null pointer");
+    SFB_REQUIRE(xyz || (rays_o && rays_d && z && T > 0), "ngp_field_normal_backward: give xyz or (rays_o, rays_d, z, T)");
+    SFB_REQUIRE((grad_fd && !grad_normal) || (grad_normal && fd && !grad_fd), "ngp_field_normal_backward: give grad_fd, or grad_normal and fd");
+    SFB_REQUIRE(eps != 0.f, "ngp_field_normal_backward: eps must not be 0");
+    const size_t smem = sizeof(FieldSmemV2Bwd) + (size_t)(kIn + 2 * kHid) * kLdB * 4;
+    SFB_ONCE_PER_DEVICE(SFB_CUDA(cudaFuncSetAttribute(field_backward_v2_kernel<StencilRows>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)));
+    const StencilRows rows{make_source(xyz, rays_o, rays_d, z, T, bound), B, eps, bound, fd, grad_normal, grad_fd};
+    const uint32_t blocks = min(rows.tiles(), (uint32_t)sm_count() * 2);
+    field_backward_v2_kernel<<<blocks, kBT, smem, as_stream(stream)>>>(rows, embeddings, offsets, FieldGeom{S, H, bound}, W0, b0, W1, b1, W2, b2,
+                                                                      grad_embeddings, gW0, gb0, gW1, gb1, gW2, gb2);
+    return check_launch("ngp_field_normal_backward");
 }
 
 uint64_t sfb_ngp_field_tape_floats(uint32_t B) {

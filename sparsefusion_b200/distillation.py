@@ -673,7 +673,7 @@ class ReferenceSceneBuilder:
 
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
-                      process_group=None, evaluate=False, visualize=False):
+                      process_group=None, evaluate=False, visualize=False, visualize_shadings=()):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -690,13 +690,17 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ``{save_dir}/render_gifs/{seq_name}.gif`` (gt | EFT image | render | gt mask | silhouette per scene view, without the EFT panel when not
     ``use_diffusion``), ``{save_dir}/render_imgs/{seq_name}/{view:03d}.jpg`` (gt | render) and ``{save_dir}/render_gifs/{seq_name}_circle.gif``
     (render | silhouette per circle view) are written; the sequence frames are the renders ``evaluate`` scores.  GIF palettes are quantised on
-    the GPU (``video.py``); Pillow writes the files.
+    the GPU (``video.py``); Pillow writes the files.  ``visualize_shadings`` (with ``visualize``), e.g. ``('normal', 'textureless')``, adds one
+    ``{save_dir}/render_gifs/{seq_name}_circle_{shading}.gif`` per listed shading of ``NeRFNetwork.forward``: the circle views rendered with
+    that shading under a headlight (``evaluate.render_views``), at ambient ratio 0.1 for the lit shadings ('lambertian', 'textureless') so the
+    geometry shows, 1.0 for 'normal' and 'albedo'.
 
     Not reproduced: the matplotlib loss plots and the periodic ``_vis.jpg`` renders (:355-388) -- logging, outside the hot path;
     ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference makes).
     ``scene_valid_region`` is accepted and unused, as in the reference's loop body (:192-195 overwrites the region with ones), and so is
     ``loss_fn_vgg`` unless ``evaluate``.  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
-    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``, ``visualize``.
+    torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``, ``visualize``,
+    ``visualize_shadings``.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     rank, world = 0, 1
@@ -708,13 +712,14 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
                          start_percep_step=1000, views_per_step=views_per_step)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
-                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize)
+                                     make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
+                                     visualize_shadings)
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
-                   evaluate=False, loss_fn_vgg=None, visualize=False):
+                   evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=()):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -723,7 +728,8 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     Scenes of one call must share image, latent and ray sizes.  With several GPUs, each rank passes its own share of the scenes.
     ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  ``evaluate`` / ``loss_fn_vgg``: each scene is scored and its
     ``{save_dir}/metrics/{seq_name}.txt`` written as ``distillation_loop(evaluate=True)`` does, scene k's render jitter keyed by ``seed + k``.
-    ``visualize``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter keyed by ``seed + k``.
+    ``visualize`` / ``visualize_shadings``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter
+    keyed by ``seed + k``.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
 
@@ -732,7 +738,7 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
-                             loss_fn_vgg, visualize)
+                             loss_fn_vgg, visualize, visualize_shadings)
 
 
 EFT_GRID_COLUMNS = 8     # cached EFT images per row of the grid the reference writes before its loop (:129-141)
@@ -749,11 +755,15 @@ def _write_eft_grid(path, eft_images, n_views):
     write_jpeg(path, to_uint8(grid)[0])
 
 
-def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_images, seed, scores=None):
+LIT_SHADING_AMBIENT = 0.1     # ambient ratio of the lit shadings' circle gifs: mostly light, so the geometry shows
+
+
+def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_images, seed, scores=None, shadings=()):
     """the reference's sequence gif, per-view jpegs and circle gif of one distilled scene (:444-493).  The sequence frames are ``scores``'
     renders (``evaluate_scene``'s, the ones the metrics come from) or, without scores, the same renders by ``render_views`` (stream 3);
     the circle frames are ``render_views`` of the circle rays with stream 4.  ``eft_images``: the scene views' cached EFT images [V,3,h,w]
-    (``use_diffusion``) or None."""
+    (``use_diffusion``) or None.  Each of ``shadings`` adds ``{seq_name}_circle_{shading}.gif``: the circle views rendered with that shading
+    (headlit, ``render_views``), one panel per frame."""
     from .evaluate import CIRCLE_STREAM, EVAL_STREAM, render_views
     from .video import to_uint8, write_gif, write_jpegs
     V = views.rgb.shape[0]
@@ -776,10 +786,16 @@ def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_image
     gif_path = f'{save_dir}/render_gifs/{seq_name}_circle.gif'
     write_gif(gif_path, to_uint8(c_image, c_sil[..., None]))                                                         # :487-490
     print('saved video', gif_path)
+    for shading in shadings:
+        ratio = 1.0 if shading in ('albedo', 'normal') else LIT_SHADING_AMBIENT
+        s_image, _ = render_views(ngp, rays_o, rays_d, (hw, hw), opt, seed=seed, stream=CIRCLE_STREAM, shading=shading, ambient_ratio=ratio)
+        gif_path = f'{save_dir}/render_gifs/{seq_name}_circle_{shading}.gif'
+        write_gif(gif_path, to_uint8(s_image))
+        print('saved video', gif_path)
 
 
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
-                      loss_fn_vgg=None, visualize=False):
+                      loss_fn_vgg=None, visualize=False, visualize_shadings=()):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
     ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
@@ -787,6 +803,9 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     import os
     from .lpips_vgg import PerceptualLoss
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
+    visualize_shadings = tuple(visualize_shadings)
+    if not all(isinstance(sh, str) and sh and '/' not in sh for sh in visualize_shadings):
+        raise ValueError(f'visualize_shadings must be shading names, got {visualize_shadings!r}')
     if visualize:
         from .video import require_pillow
         require_pillow()
@@ -841,5 +860,5 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
                     write_scene_metrics(f'{save_dir}/metrics/{seq_name}.txt', scores)                              # :434-441
                 if visualize:
                     _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circles[k], caches[k].target_eft_image if use_diffusion else None,
-                                          base_seed + k, scores)                                                    # :444-493
+                                          base_seed + k, scores, visualize_shadings)                                # :444-493
     return ngps

@@ -71,11 +71,13 @@ def image_metrics(pred: torch.Tensor, gt: torch.Tensor):
 
 
 @torch.no_grad()
-def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, seed: int, stream: int):
+def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, seed: int, stream: int, shading: str = 'albedo',
+                 ambient_ratio: float = 1.0):
     """(images [V, H, W, 3] fp32, silhouettes [V, H, W]) of V views (rays [V, H*W, 3], ``hw`` = (H, W)) with the reference's eval-mode render
     call (distillation.py:404-406, :480-482).  Its ``perturb=True`` jitter, which the reference draws from torch's unseeded global generator,
     comes from the CUDA generator seeded with ``view_seed(seed, 0, view, stream)`` inside ``torch.random.fork_rng``, so the renders are
-    reproducible and the callers' generators are left as they were.  ``ngp.training`` is restored on return."""
+    reproducible and the callers' generators are left as they were.  ``ngp.training`` is restored on return.  A shading other than 'albedo'
+    (NeRFNetwork.forward's) is lit by a headlight, light_d = safe_normalize(rays_o[v][0]), so a turntable of views does not flicker."""
     dev = rays_o.device
     if dev.type != 'cuda':
         raise RuntimeError('render_views: the rays must be CUDA tensors (no CPU fallback)')
@@ -91,8 +93,9 @@ def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, se
             for v in range(V):
                 with torch.random.fork_rng(devices=[dev]):
                     torch.cuda.manual_seed(view_seed(seed, 0, v, stream))
-                    out = ngp.render_batched(rays_o[v][None], rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=1.0,
-                                             shading='albedo', force_all_rays=True, **vars(opt))
+                    light = {} if shading == 'albedo' else {'light_d': torch.nn.functional.normalize(rays_o[v][0], dim=0, eps=1e-10)}
+                    out = ngp.render_batched(rays_o[v][None], rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=ambient_ratio,
+                                             shading=shading, force_all_rays=True, **light, **vars(opt))
                 images.append(out['image'].reshape(H, W, 3))
                 sils.append(out['weights_sum'].reshape(H, W))
             return torch.stack(images).float(), torch.stack(sils)

@@ -8,6 +8,10 @@ Same class / method names and keyword arguments (``render``, ``render_batched``,
 ``export_mesh`` runs the reference's mcubes export on the GPU (sparsefusion_b200/mesh.py: lattice query through the fused field kernel,
 Gaussian smoothing, marching cubes, OBJ); the textured xatlas/nvdiffrast export, dead code in the reference, is not provided.
 
+Every shading of the reference runs on both paths: 'albedo' (SparseFusion's) on the fused path below; 'lambertian' (any other
+string), 'textureless' and 'normal' shade the field with finite-difference normals computed as stencils inside the tiled field
+kernel (network_grid.py), and return the reference's loss_orient / loss_smooth.
+
 ``run`` is the default path (opt.cuda_ray = False, distillation.py:505).  The reference spells it as ~150 eager
 launches and evaluates the field three times (coarse, fine, colour); here it is seven kernels and every point is
 evaluated once per role (coarse density for the sampling pdf, then sigma+rgb at the 128 sorted samples), with an
@@ -25,6 +29,49 @@ from . import _lib as lib
 from . import raymarching
 
 
+def _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
+    """renderer_df.run :328-412: near/far, the 64 stratified and 64 importance depths, and sigma, rgb at the 128 sorted samples
+    -> (zs [N,128], sigma [N,128], rgb [N,128,3], nears [N], fars [N])"""
+    N = rays_o.shape[0]
+    dev = rays_o.device
+    enc = net.encoder
+    S, H, bound = float(math.log2(enc.per_level_scale)), int(enc.base_resolution), float(net.bound)
+    st = lib.stream()
+    f = lib.fptr
+    nears, fars = torch.empty(N, device=dev), torch.empty(N, device=dev)
+    zc = torch.empty(N, 64, device=dev)
+    lin = torch.linspace(0.0, 1.0, 64, device=dev)
+    lib.call('sfb_ray_coarse_z', f(rays_o), f(rays_d), f(aabb), float(min_near), f(lin), f(perturb_noise), N, 64, f(nears), f(fars), f(zc), st)
+    # the field is evaluated ONCE per sample: coarse pass (sigma + rgb at the 64 stratified depths), importance pass (the 64 new depths),
+    # then a gather into sorted order -- the values of the coarse samples are the same numbers a second evaluation would produce
+    sig_c, rgb_c = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
+    args = (f(emb), lib.iptr(enc.offsets), S, H, bound, f(w0), f(b0), f(w1), f(b1), f(w2), f(b2))
+    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zc), 64, N * 64, *args, f(sig_c), f(rgb_c), st)
+    zs, zn = torch.empty(N, 128, device=dev), torch.empty(N, 64, device=dev)
+    src_of = torch.empty(N, 128, dtype=torch.uint8, device=dev)
+    lib.call('sfb_ray_resample_ex', f(zc), f(sig_c), f(nears), f(fars), f(pdf_u), 0, N, 64, 64, f(zs), f(zn), src_of.data_ptr(), st)
+    sig_n, rgb_n = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
+    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zn), 64, N * 64, *args, f(sig_n), f(rgb_n), st)
+    sigma, rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
+    lib.call('sfb_ray_gather_sorted', src_of.data_ptr(), f(sig_c), f(rgb_c), f(sig_n), f(rgb_n), N, 128, f(sigma), f(rgb), st)
+    return zs, sigma, rgb, nears, fars
+
+
+def _field_backward_at_samples(net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0, b0, w1, b1, w2, b2):
+    """parameter gradients of <sigma, g_sigma> + <rgb, g_rgb> over the field at the [N,128] ray samples"""
+    enc = net.encoder
+    dev = rays_o.device
+    f = lib.fptr
+    B = zs.numel()
+    tape = torch.empty(lib.load().sfb_ngp_field_tape_floats(B), device=dev)
+    g_emb = torch.zeros_like(emb)
+    gw0, gb0, gw1, gb1, gw2, gb2 = (torch.zeros_like(t) for t in (w0, b0, w1, b1, w2, b2))
+    lib.call('sfb_ngp_field_backward', None, f(rays_o), f(rays_d), f(zs), 128, B, f(emb), lib.iptr(enc.offsets), float(math.log2(enc.per_level_scale)),
+             int(enc.base_resolution), float(net.bound), f(w0), f(b0), f(w1), f(b1), f(w2), f(b2), f(g_sigma), None if g_rgb is None else f(g_rgb),
+             f(g_emb), f(gw0), f(gb0), f(gw1), f(gb1), f(gw2), f(gb2), f(tape), lib.stream())
+    return g_emb, gw0, gb0, gw1, gb1, gw2, gb2
+
+
 class _RunRender(torch.autograd.Function):
     """renderer_df.run (:310-468) for shading='albedo', bg_radius == 0: returns (image [N,3], depth [N], weights_sum [N], nears, fars)"""
 
@@ -32,28 +79,10 @@ class _RunRender(torch.autograd.Function):
     def forward(ctx, net, rays_o, rays_d, aabb, min_near, bg_color, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
         N = rays_o.shape[0]
         dev = rays_o.device
-        enc = net.encoder
-        S, H, bound = float(math.log2(enc.per_level_scale)), int(enc.base_resolution), float(net.bound)
-        st = lib.stream()
         f = lib.fptr
-        nears, fars = torch.empty(N, device=dev), torch.empty(N, device=dev)
-        zc = torch.empty(N, 64, device=dev)
-        lin = torch.linspace(0.0, 1.0, 64, device=dev)
-        lib.call('sfb_ray_coarse_z', f(rays_o), f(rays_d), f(aabb), float(min_near), f(lin), f(perturb_noise), N, 64, f(nears), f(fars), f(zc), st)
-        # the field is evaluated ONCE per sample: coarse pass (sigma + rgb at the 64 stratified depths), importance pass (the 64 new depths),
-        # then a gather into sorted order -- the values of the coarse samples are the same numbers a second evaluation would produce
-        sig_c, rgb_c = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
-        args = (f(emb), lib.iptr(enc.offsets), S, H, bound, f(w0), f(b0), f(w1), f(b1), f(w2), f(b2))
-        lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zc), 64, N * 64, *args, f(sig_c), f(rgb_c), st)
-        zs, zn = torch.empty(N, 128, device=dev), torch.empty(N, 64, device=dev)
-        src_of = torch.empty(N, 128, dtype=torch.uint8, device=dev)
-        lib.call('sfb_ray_resample_ex', f(zc), f(sig_c), f(nears), f(fars), f(pdf_u), 0, N, 64, 64, f(zs), f(zn), src_of.data_ptr(), st)
-        sig_n, rgb_n = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
-        lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zn), 64, N * 64, *args, f(sig_n), f(rgb_n), st)
-        sigma, rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
-        lib.call('sfb_ray_gather_sorted', src_of.data_ptr(), f(sig_c), f(rgb_c), f(sig_n), f(rgb_n), N, 128, f(sigma), f(rgb), st)
+        zs, sigma, rgb, nears, fars = _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2)
         image, depth, ws = torch.empty(N, 3, device=dev), torch.empty(N, device=dev), torch.empty(N, device=dev)
-        lib.call('sfb_ray_composite_forward', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, 128, f(image), f(depth), f(ws), st)
+        lib.call('sfb_ray_composite_forward', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, 128, f(image), f(depth), f(ws), lib.stream())
         ctx.save_for_backward(rays_o, rays_d, zs, sigma, rgb, nears, fars, emb, w0, b0, w1, b1, w2, b2)
         ctx.net, ctx.bg = net, float(bg_color)
         ctx.mark_non_differentiable(nears, fars)
@@ -62,26 +91,71 @@ class _RunRender(torch.autograd.Function):
     @staticmethod
     def backward(ctx, g_image, g_depth, g_ws, _gn, _gf):
         rays_o, rays_d, zs, sigma, rgb, nears, fars, emb, w0, b0, w1, b1, w2, b2 = ctx.saved_tensors
-        net = ctx.net
-        enc = net.encoder
-        N = rays_o.shape[0]
-        dev = rays_o.device
-        S, H, bound = float(math.log2(enc.per_level_scale)), int(enc.base_resolution), float(net.bound)
-        st = lib.stream()
+        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws)
+        grads = _field_backward_at_samples(ctx.net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0, b0, w1, b1, w2, b2)
+        return (None, None, None, None, None, None, None, None, *grads)
+
+
+def _composite_backward(zs, sigma, rgb, nears, fars, bg, g_image, g_depth, g_ws):
+    """sfb_ray_composite_backward: (dL/dsigma [N,128], dL/drgb [N,128,3])"""
+    N = zs.shape[0]
+    dev = zs.device
+    f = lib.fptr
+    g_image = g_image.contiguous() if g_image is not None else torch.zeros(N, 3, device=dev)
+    g_sigma, g_rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
+    g_ws = None if g_ws is None else g_ws.contiguous()
+    g_depth = None if g_depth is None else g_depth.contiguous()
+    lib.call('sfb_ray_composite_backward', f(zs), f(sigma), f(rgb), f(nears), f(fars), bg, N, 128, f(g_image),
+             None if g_ws is None else f(g_ws), None if g_depth is None else f(g_depth), f(g_sigma), f(g_rgb), lib.stream())
+    return g_sigma, g_rgb
+
+
+class _RaySamples(torch.autograd.Function):
+    """the field at the 128 sorted samples of run (renderer_df.py:328-412) as an autograd node: (sigma [N,128], albedo [N,128,3], zs, nears,
+    fars); the backward runs the field backward at the same samples"""
+
+    @staticmethod
+    def forward(ctx, net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
+        zs, sigma, rgb, nears, fars = _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2)
+        ctx.save_for_backward(rays_o, rays_d, zs, emb, w0, b0, w1, b1, w2, b2)
+        ctx.net = net
+        ctx.mark_non_differentiable(zs, nears, fars)
+        return sigma, rgb, zs, nears, fars
+
+    @staticmethod
+    def backward(ctx, g_sigma, g_rgb, _gz, _gn, _gf):
+        rays_o, rays_d, zs, emb, w0, b0, w1, b1, w2, b2 = ctx.saved_tensors
+        g_sigma = torch.zeros_like(zs) if g_sigma is None else g_sigma.contiguous()
+        g_rgb = None if g_rgb is None else g_rgb.contiguous()
+        grads = _field_backward_at_samples(ctx.net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0, b0, w1, b1, w2, b2)
+        return (None, None, None, None, None, None, None, *grads)
+
+
+class _Composite(torch.autograd.Function):
+    """renderer_df.py:414-456 (bg_radius == 0): (image [N,3], depth [N], weights_sum [N]) of colours rgb [N,128,3] at depths zs"""
+
+    @staticmethod
+    def forward(ctx, zs, sigma, rgb, nears, fars, bg_color):
+        N = zs.shape[0]
+        dev = zs.device
         f = lib.fptr
-        g_image = g_image.contiguous() if g_image is not None else torch.zeros(N, 3, device=dev)
-        g_sigma, g_rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
-        g_ws = None if g_ws is None else g_ws.contiguous()
-        g_depth = None if g_depth is None else g_depth.contiguous()
-        lib.call('sfb_ray_composite_backward', f(zs), f(sigma), f(rgb), f(nears), f(fars), ctx.bg, N, 128, f(g_image),
-                 None if g_ws is None else f(g_ws), None if g_depth is None else f(g_depth), f(g_sigma), f(g_rgb), st)
-        B = N * 128
-        tape = torch.empty(lib.load().sfb_ngp_field_tape_floats(B), device=dev)
-        g_emb = torch.zeros_like(emb)
-        gw0, gb0, gw1, gb1, gw2, gb2 = (torch.zeros_like(t) for t in (w0, b0, w1, b1, w2, b2))
-        lib.call('sfb_ngp_field_backward', None, f(rays_o), f(rays_d), f(zs), 128, B, f(emb), lib.iptr(enc.offsets), S, H, bound, f(w0), f(b0), f(w1),
-                 f(b1), f(w2), f(b2), f(g_sigma), f(g_rgb), f(g_emb), f(gw0), f(gb0), f(gw1), f(gb1), f(gw2), f(gb2), f(tape), st)
-        return (None, None, None, None, None, None, None, None, g_emb, gw0, gb0, gw1, gb1, gw2, gb2)
+        sigma, rgb = sigma.contiguous(), rgb.contiguous()
+        image, depth, ws = torch.empty(N, 3, device=dev), torch.empty(N, device=dev), torch.empty(N, device=dev)
+        lib.call('sfb_ray_composite_forward', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, 128, f(image), f(depth), f(ws), lib.stream())
+        ctx.save_for_backward(zs, sigma, rgb, nears, fars)
+        ctx.bg = float(bg_color)
+        return image, depth, ws
+
+    @staticmethod
+    def backward(ctx, g_image, g_depth, g_ws):
+        zs, sigma, rgb, nears, fars = ctx.saved_tensors
+        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws)
+        return None, g_sigma, g_rgb, None, None, None
+
+
+def _safe_normalize(x, eps=1e-20):
+    """external/nerf/utils.py:41-42"""
+    return x / torch.sqrt(torch.clamp(torch.sum(x * x, -1, keepdim=True), min=eps))
 
 
 class NeRFRenderer(nn.Module):
@@ -145,12 +219,13 @@ class NeRFRenderer(nn.Module):
 
     # ------------------------------------------------------------------------------------------ default path
     def run(self, rays_o, rays_d, num_steps=128, upsample_steps=128, light_d=None, ambient_ratio=1.0, shading='albedo', bg_color=None,
-            perturb=False, fixed_light=False, perturb_noise=None, pdf_noise=None, **kwargs):
-        """rays_o, rays_d: [B, N, 3] (B == 1) -> image [B,N,3], depth [B,N], weights_sum [N], mask [B,N].
-        ``perturb_noise`` [N,num_steps] / ``pdf_noise`` [N,upsample_steps] override the torch.rand draws (parity tests)."""
-        if shading != 'albedo' or self.bg_radius > 0:
-            raise NotImplementedError("the fused renderer covers SparseFusion's configuration: shading='albedo', bg_radius=0 "
-                                      '(sparsefusion/distillation.py:209,512)')
+            perturb=False, fixed_light=False, perturb_noise=None, pdf_noise=None, normal_noise=None, regularisers=True, **kwargs):
+        """rays_o, rays_d: [B, N, 3] (B == 1) -> image [B,N,3], depth [B,N], weights_sum [N], mask [B,N], and with a shading other than
+        'albedo' loss_orient and loss_smooth (:427-436).  ``perturb_noise`` [N,num_steps] / ``pdf_noise`` [N,upsample_steps] /
+        ``normal_noise`` [N,128,3] override the torch.rand / torch.randn draws (parity tests).  ``regularisers=False`` skips loss_orient and
+        loss_smooth (and the randn of :434 with them): ``render(staged=True)`` passes it, since the reference discards them there."""
+        if self.bg_radius > 0:
+            raise NotImplementedError("the fused renderer covers SparseFusion's configuration: bg_radius=0 (sparsefusion/distillation.py:512)")
         if num_steps != 64 or upsample_steps != 64:
             raise NotImplementedError('the fused renderer is built for num_steps = upsample_steps = 64 (get_default_torch_ngp_opt)')
         prefix = rays_o.shape[:-1]
@@ -166,6 +241,12 @@ class NeRFRenderer(nn.Module):
         if not isinstance(bg_color, (int, float)):
             raise NotImplementedError('per-ray bg_color tensors are not used by the distillation loop (bg_color=0)')
         with torch.cuda.device(dev):
+            if shading != 'albedo' and light_d is None:                                         # :333-352, drawn first as there
+                if fixed_light:
+                    rot_m = torch.tensor([[0.63, .65, -0.43], [-.43, .75, -0.5], [-.65, .13, .75]], device=dev, dtype=torch.float)
+                    light_d = _safe_normalize(rays_o[0] @ rot_m)
+                else:
+                    light_d = _safe_normalize(rays_o[0] + torch.randn(3, device=dev, dtype=torch.float))
             if perturb and perturb_noise is None:
                 perturb_noise = torch.rand(N, num_steps, device=dev)                          # renderer_df.py:363
             if not perturb:
@@ -177,6 +258,9 @@ class NeRFRenderer(nn.Module):
             pdf_u = pdf_u.contiguous()
             p = self._field_params()
             pn = None if perturb_noise is None else perturb_noise.contiguous()
+            if shading != 'albedo':
+                return self._run_shaded(rays_o, rays_d, prefix, aabb, bg_color, pn, pdf_u, light_d, ambient_ratio, shading, normal_noise,
+                                        regularisers)
             if N <= self.MAX_RAYS_PER_LAUNCH:
                 image, depth, ws, nears, fars = _RunRender.apply(self, rays_o, rays_d, aabb, self.min_near, bg_color, pn, pdf_u, *p)
             else:
@@ -188,6 +272,54 @@ class NeRFRenderer(nn.Module):
                 image, depth, ws, nears, fars = (torch.cat([q[j] for q in parts]) for j in range(5))
         return {'image': image.view(*prefix, 3), 'depth': depth.view(*prefix), 'weights_sum': ws, 'mask': (nears < fars).reshape(*prefix)}
 
+    def _run_shaded(self, rays_o, rays_d, prefix, aabb, bg_color, pn, pdf_u, light_d, ratio, shading, normal_noise, regularisers):
+        """run with a normal-based shading, in slices of MAX_RAYS_PER_LAUNCH rays as the albedo path (each slice its own autograd nodes, so
+        the v1 field kernels' backward tape exists for one slice at a time); the regularisers are means over all slices' samples"""
+        N = rays_o.shape[0]
+        M = self.MAX_RAYS_PER_LAUNCH
+        parts = [self._shade_slice(rays_o[i:i + M], rays_d[i:i + M], aabb, bg_color, None if pn is None else pn[i:i + M], pdf_u[i:i + M], light_d,
+                                   ratio, shading, None if normal_noise is None else normal_noise[i:i + M], regularisers) for i in range(0, N, M)]
+        image, depth, ws, nears, fars = (torch.cat([q[j] for q in parts]) for j in range(5))
+        out = {'image': image.view(*prefix, 3), 'depth': depth.view(*prefix), 'weights_sum': ws, 'mask': (nears < fars).reshape(*prefix)}
+        if regularisers:
+            out['loss_orient'] = sum(q[5] for q in parts) / (N * 128)
+            out['loss_smooth'] = sum(q[6] for q in parts) / (N * 128 * 3)
+        return out
+
+    def _shade_slice(self, rays_o, rays_d, aabb, bg_color, pn, pdf_u, light_d, ratio, shading, normal_noise, regularisers):
+        """one slice of rays: the field at the 128 sorted samples (one autograd node), the normal there (the smoothed stencil for 'textureless'
+        / 'normal', the plain one with gradient otherwise), shading (network_grid.py:187-195), compositing, and the sums of the orientation and
+        smoothness terms (renderer_df.py:427-436, with the weights of :416-418, detached) -> (image, depth, ws, nears, fars, orient, smooth)"""
+        from .network_grid import _NormalFn, shade, stencil_forward, jitter_key
+        N = rays_o.shape[0]
+        dev = rays_o.device
+        p = self._field_params()
+        sigma, albedo, zs, nears, fars = _RaySamples.apply(self, rays_o, rays_d, aabb, self.min_near, pn, pdf_u, *p)
+        rays = (rays_o, rays_d, zs)
+        if shading in ('textureless', 'normal'):
+            with torch.no_grad():
+                normal = stencil_forward(self, N * 128, rays=rays, k=10, eps=3e-1, radius=3e-1, key=jitter_key(dev), want_fd=False)[1]
+        else:
+            normal = _NormalFn.apply(self, None, rays, 1e-2, True, *p)
+        color, _ = shade(albedo.view(-1, 3), normal, light_d, ratio, shading)
+        image, depth, ws = _Composite.apply(zs, sigma, color.view(N, 128, 3), nears, fars, bg_color)
+        if not regularisers:
+            return image, depth, ws, nears, fars
+        with torch.no_grad():
+            sample_dist = ((fars - nears) / 64)[:, None]
+            deltas = torch.cat([zs[:, 1:] - zs[:, :-1], sample_dist], -1)
+            alphas = 1 - torch.exp(-deltas * sigma)
+            weights = alphas * torch.cumprod(torch.cat([torch.ones_like(alphas[:, :1]), 1 - alphas + 1e-15], -1), -1)[:, :-1]
+            xyzs = torch.min(torch.max(rays_o[:, None, :] + rays_d[:, None, :] * zs[..., None], aabb[:3]), aabb[3:])
+            if normal_noise is None:
+                normal_noise = torch.randn_like(xyzs)
+        normals = normal.view(N, 128, 3)
+        dirs = rays_d.view(-1, 1, 3).expand_as(normals)
+        orient = (weights * (normals * dirs).sum(-1).clamp(min=0) ** 2).sum()
+        normals_perturb = self.normal(xyzs + normal_noise.to(dev) * 1e-2).view(N, 128, 3)
+        smooth = (normals - normals_perturb).abs().sum()
+        return image, depth, ws, nears, fars, orient, smooth
+
     # ------------------------------------------------------------------------------------------ cuda_ray path
     def run_cuda(self, rays_o, rays_d, dt_gamma=0, light_d=None, ambient_ratio=1.0, shading='albedo', bg_color=None, perturb=False,
                  force_all_rays=False, max_steps=1024, T_thresh=1e-4, **kwargs):
@@ -198,6 +330,8 @@ class NeRFRenderer(nn.Module):
         device = rays_o.device
         # NB: like the reference (renderer_df.py:483) min_near is NOT forwarded here -> the wrapper default 0.2
         nears, fars = raymarching.near_far_from_aabb(rays_o, rays_d, self.aabb_train if self.training else self.aabb_infer)
+        if shading != 'albedo' and light_d is None:       # :486-489
+            light_d = _safe_normalize(rays_o[0] + torch.randn(3, device=device, dtype=torch.float))
         results = {}
         if self.training:
             counter = self.step_counter[self.local_step % 16]
@@ -206,8 +340,13 @@ class NeRFRenderer(nn.Module):
             xyzs, dirs, deltas, rays = raymarching.march_rays_train(rays_o, rays_d, self.bound, self.density_bitfield, self.cascade, self.grid_size,
                                                                     nears, fars, counter, self.mean_count, perturb, 128, force_all_rays, dt_gamma,
                                                                     max_steps)
-            sigmas, rgbs, _ = self(xyzs, dirs, light_d, ratio=ambient_ratio, shading=shading)
+            sigmas, rgbs, normals = self(xyzs, dirs, light_d, ratio=ambient_ratio, shading=shading)
             weights_sum, depth, image = raymarching.composite_rays_train(sigmas, rgbs, deltas, rays, T_thresh)
+            if normals is not None:                       # :509-519, with the weights 1 - exp(-sigma) used there
+                weights = 1 - torch.exp(-sigmas)
+                results['loss_orient'] = (weights.detach() * (normals * dirs).sum(-1).clamp(min=0) ** 2).mean()
+                normals_perturb = self.normal(xyzs + torch.randn_like(xyzs) * 1e-2)
+                results['loss_smooth'] = (normals - normals_perturb).abs().mean()
         else:
             weights_sum = torch.zeros(N, dtype=torch.float32, device=device)
             depth = torch.zeros(N, dtype=torch.float32, device=device)
@@ -287,7 +426,8 @@ class NeRFRenderer(nn.Module):
                 head = 0
                 while head < N:
                     tail = min(head + max_ray_batch, N)
-                    r = _run(rays_o[b:b + 1, head:tail], rays_d[b:b + 1, head:tail], **kwargs)
+                    # only three keys survive here (as in the reference), so the shaded path's regularisers are not computed
+                    r = _run(rays_o[b:b + 1, head:tail], rays_d[b:b + 1, head:tail], regularisers=False, **kwargs)
                     depth[b:b + 1, head:tail] = r['depth']
                     weights_sum[b:b + 1, head:tail] = r['weights_sum']
                     image[b:b + 1, head:tail] = r['image']
