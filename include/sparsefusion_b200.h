@@ -400,6 +400,25 @@ int sfb_grid_sample_nhwc(const float* x, int64_t ldx, const float* grid, float* 
 int sfb_seq_attention(const float* qkv, float* out, int S, int B, int E, void* stream);
 /* in place over n floats (n % 4 == 0): kind 0 ReLU, 1 GELU (erf) */
 int sfb_act_inplace(float* x, int64_t n, int kind, void* stream);
+/* the T1 token rows of the view-batched feature cache (eft.py:215-327, what EpipolarFeatureTransformer.forward assembles in eager passes), for
+ * V query views with their own NC input cameras each: cams [V][NC][16] = R row-major (9) | T (3) | focal (2) | principal point (2) in pytorch3d's
+ * NDC row-vector convention; origins / directions [V][N][3], lengths [V][N][D]; latent [NC][h][w] (channel stride ldl, C channels) and images
+ * [NC][H][W] (channel stride ldi, Ci channels) NHWC.  Row (c, v, n, d) of out [NC][V*N*D][ldo] (ldo >= 91 + C + Ci) gets, for the point
+ * x = o + l d: the reference Pluecker harmonic embedding (78) of (u, centre_c x u), u = normalize(x - centre_c); the depth harmonic embedding
+ * (13) of l; the bilinear look-ups (sfb_grid_sample_nhwc semantics) of the latent and the images at minus the NDC projection of x by camera
+ * (v, c); zeros up to ldo.  Harmonics: [sin(x f_k), cos(x f_k), x], f_k = omega0 2^k, k < 6. */
+int sfb_eft_t1_tokens(const float* cams, const float* origins, const float* directions, const float* lengths, const float* latent, int64_t ldl,
+                      int h, int w, int C, const float* images, int64_t ldi, int H, int W, int Ci, float omega0, float* out, int64_t ldo, int V,
+                      int NC, int N, int D, void* stream);
+
+/* ==========================================================================================
+ * section 8b -- ray grids of the per-scene preparation (sparsefusion/distillation.py:85-86 through utils/render_utils.py:16-65)
+ * ========================================================================================== */
+/* pytorch3d GridRaysampler rays of V cameras in one launch: cams [V][16] as for sfb_eft_t1_tokens; the H x W NDC grid x_j = linspace(min_x,
+ * max_x, W)[j], y_i = linspace(min_y, max_y, H)[i]; p1, p2 = the pixel unprojected at depths 1 and 2; rays_d = p2 - p1 (not normalised),
+ * rays_o = p1 - rays_d; rays_o / rays_d [V][H*W][3], row-major pixels (_xy_to_ray_bundle). */
+int sfb_grid_rays(const float* cams, int V, int H, int W, float min_x, float max_x, float min_y, float max_y, float* rays_o, float* rays_d,
+                  void* stream);
 
 /* ==========================================================================================
  * section 9 -- mesh extraction from a density lattice (NeRFRenderer.export_mesh, external/nerf/renderer_df.py:121-153)

@@ -62,6 +62,33 @@ __global__ void resize_bilinear_ac_kernel(const float* __restrict__ x, int64_t l
     }
 }
 
+// F.grid_sample(mode='bilinear', padding_mode='border', align_corners=True) at one point (gx, gy) in [-1, 1] of an NHWC image b [H][W]
+// (channel stride ldx): the four corner rows and their weights.  Out-of-range corners contribute zero (their weight is zero anyway).
+struct BorderBilinear {
+    const float *p00, *p01, *p10, *p11;
+    float w00, w01, w10, w11;
+    __device__ __forceinline__ float operator()(int c) const {
+        return __ldg(p00 + c) * w00 + __ldg(p01 + c) * w01 + __ldg(p10 + c) * w10 + __ldg(p11 + c) * w11;
+    }
+};
+
+__device__ __forceinline__ BorderBilinear border_bilinear(const float* b, int64_t ldx, int H, int W, float gx, float gy) {
+    float ix = (gx + 1.f) * 0.5f * (W - 1), iy = (gy + 1.f) * 0.5f * (H - 1);      // grid_sampler_unnormalize, align_corners
+    ix = fminf(fmaxf(ix, 0.f), (float)(W - 1));                                     // clip_coordinates (border)
+    iy = fminf(fmaxf(iy, 0.f), (float)(H - 1));
+    const float fx0 = floorf(ix), fy0 = floorf(iy);
+    const int x0 = (int)fx0, y0 = (int)fy0, x1 = x0 + 1, y1 = y0 + 1;
+    const float wx1 = ix - fx0, wy1 = iy - fy0, wx0 = 1.f - wx1, wy0 = 1.f - wy1;
+    const bool vx1 = x1 <= W - 1, vy1 = y1 <= H - 1;
+    BorderBilinear s;
+    s.p00 = b + ((int64_t)y0 * W + x0) * ldx;
+    s.p01 = b + ((int64_t)y0 * W + (vx1 ? x1 : x0)) * ldx;
+    s.p10 = b + ((int64_t)(vy1 ? y1 : y0) * W + x0) * ldx;
+    s.p11 = b + ((int64_t)(vy1 ? y1 : y0) * W + (vx1 ? x1 : x0)) * ldx;
+    s.w00 = wx0 * wy0; s.w01 = vx1 ? wx1 * wy0 : 0.f; s.w10 = vy1 ? wx0 * wy1 : 0.f; s.w11 = (vx1 && vy1) ? wx1 * wy1 : 0.f;
+    return s;
+}
+
 // F.grid_sample(x, grid, mode='bilinear', padding_mode='border', align_corners=True) with NHWC input and point-major output:
 // out[n][m][c] = bilinear(x[n], grid[n][m] = (gx, gy) in [-1, 1]).  One warp per point, lanes over channels (scalar channels: C need not be a
 // multiple of 4 -- the RGB look-up has 3).  eft.py:248-275.
@@ -71,22 +98,77 @@ __global__ void grid_sample_kernel(const float* __restrict__ x, int64_t ldx, con
     if (pt >= total_pts) return;
     const int lane = threadIdx.x & 31;
     const int n = (int)(pt / M);
-    const float gx = __ldg(grid + pt * 2), gy = __ldg(grid + pt * 2 + 1);
-    float ix = (gx + 1.f) * 0.5f * (W - 1), iy = (gy + 1.f) * 0.5f * (H - 1);      // grid_sampler_unnormalize, align_corners
-    ix = fminf(fmaxf(ix, 0.f), (float)(W - 1));                                     // clip_coordinates (border)
-    iy = fminf(fmaxf(iy, 0.f), (float)(H - 1));
-    const float fx0 = floorf(ix), fy0 = floorf(iy);
-    const int x0 = (int)fx0, y0 = (int)fy0, x1 = x0 + 1, y1 = y0 + 1;
-    const float wx1 = ix - fx0, wy1 = iy - fy0, wx0 = 1.f - wx1, wy0 = 1.f - wy1;
-    const bool vx1 = x1 <= W - 1, vy1 = y1 <= H - 1;                                // out-of-range corners contribute zero (their weight is zero anyway)
-    const float* b = x + (int64_t)n * H * W * ldx;
-    const float* p00 = b + ((int64_t)y0 * W + x0) * ldx;
-    const float* p01 = b + ((int64_t)y0 * W + (vx1 ? x1 : x0)) * ldx;
-    const float* p10 = b + ((int64_t)(vy1 ? y1 : y0) * W + x0) * ldx;
-    const float* p11 = b + ((int64_t)(vy1 ? y1 : y0) * W + (vx1 ? x1 : x0)) * ldx;
-    const float w00 = wx0 * wy0, w01 = vx1 ? wx1 * wy0 : 0.f, w10 = vy1 ? wx0 * wy1 : 0.f, w11 = (vx1 && vy1) ? wx1 * wy1 : 0.f;
+    const BorderBilinear s = border_bilinear(x + (int64_t)n * H * W * ldx, ldx, H, W, __ldg(grid + pt * 2), __ldg(grid + pt * 2 + 1));
     float* o = out + pt * ldo;
-    for (int c = lane; c < C; c += 32) o[c] = __ldg(p00 + c) * w00 + __ldg(p01 + c) * w01 + __ldg(p10 + c) * w10 + __ldg(p11 + c) * w11;
+    for (int c = lane; c < C; c += 32) o[c] = s(c);
+}
+
+// column j of HarmonicEmbedding (utils/common_utils.py:68-140, 6 frequencies f_k = omega0 2^k) over n coordinates v: sin of all (coordinate,
+// k) pairs coordinate-major, then cos of all, then the coordinates themselves.  v is indexed by an unrolled select, so it stays in registers.
+template <int n>
+__device__ __forceinline__ float harmonic(const float (&v)[n], int j, float omega0) {
+    constexpr int nf = 6 * n;
+    const int q = j >= 2 * nf ? j - 2 * nf : (j % nf) / 6;
+    float x = v[0];
+#pragma unroll
+    for (int i = 1; i < n; ++i) x = q == i ? v[i] : x;
+    if (j >= 2 * nf) return x;
+    const float a = x * ((float)(1 << (j % nf % 6)) * omega0);
+    return j < nf ? sinf(a) : cosf(a);
+}
+
+// T1 token rows of the view-batched EFT feature cache: one warp per (camera c, view v, ray n, depth d) row, lanes over the row's columns.
+// The point, its projection and the camera centre are computed by every lane (a few dozen flops); each of the row's 91 embedding columns by
+// one lane; the latent / image look-ups lanes-over-channels like grid_sample_kernel.  Arithmetic in the order of the eager assembly in
+// EpipolarFeatureTransformer.forward (no FMA contraction where the eager ops round twice).
+__global__ void __launch_bounds__(256) eft_t1_tokens_kernel(const float* __restrict__ cams, const float* __restrict__ origins,
+                                                            const float* __restrict__ directions, const float* __restrict__ lengths,
+                                                            const float* __restrict__ latent, int64_t ldl, int h, int w, int C,
+                                                            const float* __restrict__ images, int64_t ldi, int H, int W, int Ci, float omega0,
+                                                            float* __restrict__ out, int64_t ldo, int V, int NC, int N, int D) {
+    const int64_t VND = (int64_t)V * N * D;
+    const int64_t row = blockIdx.x * (int64_t)(blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= (int64_t)NC * VND) return;
+    const int lane = threadIdx.x & 31;
+    const int c = (int)(row / VND);
+    const int64_t r = row % VND;                       // (v, n, d)
+    const int64_t ray = r / D;                         // v * N + n
+    const int v = (int)(ray / N);
+    const float* cam = cams + ((int64_t)v * NC + c) * 16;
+    float R[9], T[3];
+#pragma unroll
+    for (int i = 0; i < 9; ++i) R[i] = __ldg(cam + i);
+#pragma unroll
+    for (int i = 0; i < 3; ++i) T[i] = __ldg(cam + 9 + i);
+    const float l = __ldg(lengths + r);
+    float x[3], oc[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) x[i] = __fadd_rn(__ldg(origins + ray * 3 + i), __fmul_rn(l, __ldg(directions + ray * 3 + i)));
+#pragma unroll
+    for (int i = 0; i < 3; ++i) oc[i] = -(T[0] * R[i * 3 + 0] + T[1] * R[i * 3 + 1] + T[2] * R[i * 3 + 2]);     // centre = -T R^T
+    // reference Pluecker coordinates (u, oc x u), u = normalize(x - oc) (F.normalize, eps 1e-12)
+    float u[3] = {__fsub_rn(x[0], oc[0]), __fsub_rn(x[1], oc[1]), __fsub_rn(x[2], oc[2])};
+    const float nrm = fmaxf(sqrtf(u[0] * u[0] + u[1] * u[1] + u[2] * u[2]), 1e-12f);
+    float pl[6];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) pl[i] = u[i] / nrm;
+    pl[3] = __fsub_rn(__fmul_rn(oc[1], pl[2]), __fmul_rn(oc[2], pl[1]));
+    pl[4] = __fsub_rn(__fmul_rn(oc[2], pl[0]), __fmul_rn(oc[0], pl[2]));
+    pl[5] = __fsub_rn(__fmul_rn(oc[0], pl[1]), __fmul_rn(oc[1], pl[0]));
+    float* o = out + row * ldo;
+    const float lv[1] = {l};
+    for (int j = lane; j < 91; j += 32) o[j] = j < 78 ? harmonic(pl, j, omega0) : harmonic(lv, j - 78, omega0);
+    // NDC projection by camera (v, c): x_view = x R + T, ndc = f x_view.xy / z + p; look-ups at -ndc (eft.py:241-272)
+    float xv[3];
+#pragma unroll
+    for (int i = 0; i < 3; ++i) xv[i] = x[0] * R[0 * 3 + i] + x[1] * R[1 * 3 + i] + x[2] * R[2 * 3 + i] + T[i];
+    const float gx = -(__ldg(cam + 12) * xv[0] / xv[2] + __ldg(cam + 14));
+    const float gy = -(__ldg(cam + 13) * xv[1] / xv[2] + __ldg(cam + 15));
+    const BorderBilinear sl = border_bilinear(latent + (int64_t)c * h * w * ldl, ldl, h, w, gx, gy);
+    for (int k = lane; k < C; k += 32) o[91 + k] = sl(k);
+    const BorderBilinear si = border_bilinear(images + (int64_t)c * H * W * ldi, ldi, H, W, gx, gy);
+    for (int k = lane; k < Ci; k += 32) o[91 + C + k] = si(k);
+    for (int64_t k = 91 + C + Ci + lane; k < ldo; k += 32) o[k] = 0.f;
 }
 
 // nn.MultiheadAttention core, ONE head, sequence-first layout (nn.TransformerEncoderLayer default): qkv [S][B][3E] (in_proj output: q | k | v),
@@ -186,6 +268,19 @@ int sfb_grid_sample_nhwc(const float* x, int64_t ldx, const float* grid, float* 
     if (pts == 0 || C == 0) return SFB_OK;
     grid_sample_kernel<<<(unsigned)ceil_div(pts, (int64_t)8), 256, 0, as_stream(stream)>>>(x, ldx, grid, out, ldo, H, W, C, M, pts);
     return check_launch("grid_sample");
+}
+
+int sfb_eft_t1_tokens(const float* cams, const float* origins, const float* directions, const float* lengths, const float* latent, int64_t ldl,
+                      int h, int w, int C, const float* images, int64_t ldi, int H, int W, int Ci, float omega0, float* out, int64_t ldo, int V,
+                      int NC, int N, int D, void* stream) {
+    SFB_REQUIRE(cams && origins && directions && lengths && latent && images && out, "eft_t1_tokens: null pointer");
+    SFB_REQUIRE(ldo >= 91 + C + Ci && ldl >= C && ldi >= Ci, "eft_t1_tokens: row stride below 91 + C + Ci, or a channel stride below its channel count");
+    SFB_REQUIRE(h >= 1 && w >= 1 && H >= 1 && W >= 1, "eft_t1_tokens: empty latent or image");
+    const int64_t rows = (int64_t)NC * V * N * D;
+    if (rows == 0) return SFB_OK;
+    eft_t1_tokens_kernel<<<(unsigned)ceil_div(rows, (int64_t)8), 256, 0, as_stream(stream)>>>(cams, origins, directions, lengths, latent, ldl, h, w, C,
+                                                                                              images, ldi, H, W, Ci, omega0, out, ldo, V, NC, N, D);
+    return check_launch("eft_t1_tokens");
 }
 
 int sfb_seq_attention(const float* qkv, float* out, int S, int B, int E, void* stream) {

@@ -671,6 +671,71 @@ class ReferenceSceneBuilder:
         return self._grid_rays(scene_cameras, circle_n=n)
 
 
+class NativeSceneBuilder:
+    """``ReferenceSceneBuilder`` without pytorch3d or the reference tree: the same protocol (``build``, ``eval_views``, ``circle_views``) and
+    the same ``SceneCache`` / ``EvalViews`` contents in the same view order, following distillation.py:65-125 step by step.  The camera maths
+    runs on the host (``cameras.py``: relative / voxel-frame cameras, the 50 jittered circle-path cameras drawn with ``torch.rand`` from
+    torch's global generator as the reference draws them), every ray grid of a call in one ``sfb_grid_rays`` launch, and the EFT feature
+    cache of all (scene + circle) views through ``EpipolarFeatureTransformer.feature_cache`` -- the ResNet-18 pyramid once per scene instead
+    of twice per view.  ``scene_cameras``: pytorch3d-style cameras (any object with R, T, focal_length, principal_point, image_size)."""
+
+    RAYS_HW = 128           # sampler_feat: 256 // 2 (:85)
+    EFT_HW = 32             # renderer_feat: 256 // 8, 20 points per ray (:86; utils/render_utils.py:133-144)
+    EFT_DEPTHS = 20
+    EVAL_HW = 256           # sampler_grid (:85)
+    IMAGE_HW = 256          # every grid's pixel centres are those of the 256 x 256 image (utils/render_utils.py:38-41)
+
+    def __init__(self, gpu):
+        self.gpu = gpu
+        self.device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
+
+    def _rays(self, cams, hw):
+        from .cameras import grid_rays
+        return grid_rays(cams, hw, hw, self.device, self.IMAGE_HW, self.IMAGE_HW)
+
+    def build(self, eft, scene_cameras, scene_rgb, scene_mask, input_idx, use_diffusion=True) -> 'SceneCache':
+        from . import cameras as C
+        cams = C.as_cameras(scene_cameras).cpu()
+        input_idx = [int(i) for i in input_idx]
+        vox = C.relative_cameras(cams, [0], center_at_origin=False)                                                  # :70
+        in_o, in_d = self._rays(C.camera_slice(vox, input_idx), self.RAYS_HW)                                        # :201-204
+        dev = self.device
+        n_rays = self.RAYS_HW * self.RAYS_HW
+        empty = lambda *s: torch.zeros(0, *s, device=dev)
+        feats, eft_imgs, t_o, t_d = empty(256, self.EFT_HW, self.EFT_HW), empty(3, self.IMAGE_HW, self.IMAGE_HW), empty(n_rays, 3), empty(n_rays, 3)
+        if use_diffusion:
+            aug = C.concat_cameras([cams, C.interpolated_path(cams, n=50, theta_offset_max=0.17)])                   # :73-74
+            aug_rel = C.relative_cameras(aug, [0], center_at_origin=True)                                            # :75
+            aug_vox = C.relative_cameras(aug, [0], center_at_origin=False)                                           # :76
+            cam_dist_mean = torch.mean(torch.linalg.norm(cams.get_camera_center(), axis=1))                          # :82-84
+            V = len(aug_rel)
+            per_view = [C.relative_cameras(aug_rel, [ci], center_at_origin=True) for ci in range(V)]                 # :98 relative_cam(..., query_idx=[ci])
+            q_o, q_d = self._rays(C.concat_cameras([c[ci] for ci, c in enumerate(per_view)]), self.EFT_HW)
+            lengths = torch.linspace(float(cam_dist_mean - 5.0), float(cam_dist_mean + 5.0), self.EFT_DEPTHS, device=dev)
+            context = [c[input_idx] for c in per_view]                                                               # input_cameras of view ci (:98)
+            input_rgb = scene_rgb[input_idx].to(dev)                                                                 # scene_rgb_aug[input_idx] (:77-79, :98)
+            feats, lr = eft.feature_cache(q_o, q_d, lengths.expand(V, q_o.shape[1], -1), context, input_rgb, (self.EFT_HW, self.EFT_HW))   # :99-116
+            eft_imgs = F.interpolate(lr, scale_factor=float(self.IMAGE_HW // self.EFT_HW), mode='bilinear')          # :118-119
+            t_o, t_d = self._rays(aug_vox, self.RAYS_HW)                                                             # :115, :274-277
+        return SceneCache(input_rgb=scene_rgb[input_idx].float(), input_mask=scene_mask[input_idx].float(), input_rays_o=in_o, input_rays_d=in_d,
+                          target_features=feats, target_eft_image=eft_imgs, target_rays_o=t_o, target_rays_d=t_d)
+
+    def eval_views(self, scene_cameras, scene_rgb, scene_mask):
+        """``ReferenceSceneBuilder.eval_views``: every scene camera in the voxel frame (:70) through the 256 x 256 grid (:85, :393-406)"""
+        from . import cameras as C
+        from .evaluate import EvalViews
+        vox = C.relative_cameras(C.as_cameras(scene_cameras).cpu(), [0], center_at_origin=False)
+        o, d = self._rays(vox, self.EVAL_HW)
+        return EvalViews(rays_o=o, rays_d=d, rgb=scene_rgb.float(), mask=scene_mask.float())
+
+    def circle_views(self, scene_cameras, n=50):
+        """``ReferenceSceneBuilder.circle_views``: ``get_interpolated_path(scene_cameras_vox, n, method='circle')`` (no jitter) through the
+        256 x 256 grid (:461-469) -> (rays_o, rays_d), each [n, 256*256, 3]"""
+        from . import cameras as C
+        vox = C.relative_cameras(C.as_cameras(scene_cameras).cpu(), [0], center_at_origin=False)
+        return self._rays(C.interpolated_path(vox, n=n), self.EVAL_HW)
+
+
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
                       process_group=None, evaluate=False, visualize=False, visualize_shadings=()):

@@ -295,39 +295,7 @@ class EpipolarFeatureTransformer(nn.Module):
             tok1[..., 78:91] = depths.reshape(1, M, 13)
             # ---- T1: sequence = input views, batch = ray samples
             f1 = self._transformer('t1', tok1.view(NC * M, d1p), NC, M)                                  # zero pad columns meet zero pad weights                      # [NC*M,256]
-            # ---- T2: sequence = depth samples, batch = (view, ray)
-            d2 = (2 if self.use_r else 1) * 78 + 13 + 256
-            d2p = (d2 + 3) // 4 * 4
-            tok2 = torch.zeros(D, NC * N, d2p, dtype=torch.float32, device=dev)
-            t2v = tok2.view(D, NC, N, d2p)
-            t2v[..., :78] = query_plucker[None, None]
-            o = 78
-            if self.use_r:
-                t2v[..., o:o + 78] = ref_plucker.permute(2, 0, 1, 3)
-                o += 78
-            t2v[..., o:o + 13] = depths.permute(1, 0, 2)[:, None]
-            t2v[..., o + 13:o + 13 + 256] = f1.view(NC, N, D, 256).permute(2, 0, 1, 3)
-            f2 = self._transformer('t2', tok2.view(D * NC * N, d2p), D, NC * N).view(D, NC, N, 256)
-            sd = self._plan['sd']
-            t2 = torch.einsum('dcnf,f->dcn', f2, sd['t2_attn.weight'][0]) + sd['t2_attn.bias']      # Linear(256, 1)
-            t2_w = torch.softmax(t2, dim=0)                                                          # over the depth samples (eft.py:415)
-            f2 = (f2 * t2_w[..., None]).sum(dim=0)                                                   # [NC,N,256]
-            # ---- T3: sequence = input views, batch = rays
-            d3 = (2 if self.use_r else 1) * 78 + 256
-            d3p = (d3 + 3) // 4 * 4
-            tok3 = torch.zeros(NC, N, d3p, dtype=torch.float32, device=dev)
-            tok3[..., :78] = query_plucker[None]
-            o = 78
-            if self.use_r:
-                tok3[..., o:o + 78] = ref_plucker[:, :, D // 2, :]
-                o += 78
-            tok3[..., o:o + 256] = f2
-            f3 = self._transformer('t3', tok3.view(NC * N, d3p), NC, N).view(NC, N, 256)
-            t3_w = torch.softmax(torch.einsum('cnf,f->cn', f3, sd['t3_attn.weight'][0]) + sd['t3_attn.bias'], dim=0)   # over the views (eft.py:436)
-            f3 = (f3 * t3_w[..., None]).sum(dim=0)                                                   # [N,256]
-            rgb = f3 @ sd['color_layer.0.weight'].t() + sd['color_layer.0.bias']
-            if self.out_sigmoid:
-                rgb = torch.sigmoid(rgb)
+            rgb, f3, t2_w, t3_w = self._heads(tok1, f1, query_plucker, NC, N, D)
             if self.return_features:
                 return rgb.view(*lead, -1), f3.view(*lead, -1), 0
             ref_rgb = tok1[..., fo + self.feat_size:fo + self.feat_size + 3].view(NC, N, D, 3)       # get_coarse_rgb (eft.py:316-328)
@@ -335,6 +303,49 @@ class EpipolarFeatureTransformer(nn.Module):
             if return_intermediates:
                 return rgb, coarse, t2_w.permute(1, 2, 0)[..., None], t3_w[..., None]
             return rgb.view(*lead, -1), coarse.view(*lead, -1), 0
+
+    def _heads(self, tok1, f1, query_plucker, NC: int, N: int, D: int):
+        """everything after T1 (eft.py:396-470): T2 over the depth samples, its softmax pool, T3 over the input views, its softmax pool and the
+        colour head.  tok1 [NC, N*D, >= 91] are T1's token rows, whose first 91 columns hold the reference Pluecker embedding (78) and the depth
+        embedding (13) T2 / T3 reuse; f1 [NC*N*D, 256] is T1's output; query_plucker [N, 78].  Returns (rgb [N,3], f3 [N,256], t2_w [D,NC,N],
+        t3_w [NC,N])."""
+        dev = f1.device
+        ref_plucker = tok1[..., :78].view(NC, N, D, 78)
+        depths = tok1[0, :, 78:91].view(N, D, 13)
+        # ---- T2: sequence = depth samples, batch = (view, ray)
+        d2 = (2 if self.use_r else 1) * 78 + 13 + 256
+        d2p = (d2 + 3) // 4 * 4
+        tok2 = torch.zeros(D, NC * N, d2p, dtype=torch.float32, device=dev)
+        t2v = tok2.view(D, NC, N, d2p)
+        t2v[..., :78] = query_plucker[None, None]
+        o = 78
+        if self.use_r:
+            t2v[..., o:o + 78] = ref_plucker.permute(2, 0, 1, 3)
+            o += 78
+        t2v[..., o:o + 13] = depths.permute(1, 0, 2)[:, None]
+        t2v[..., o + 13:o + 13 + 256] = f1.view(NC, N, D, 256).permute(2, 0, 1, 3)
+        f2 = self._transformer('t2', tok2.view(D * NC * N, d2p), D, NC * N).view(D, NC, N, 256)
+        sd = self._plan['sd']
+        t2 = torch.einsum('dcnf,f->dcn', f2, sd['t2_attn.weight'][0]) + sd['t2_attn.bias']      # Linear(256, 1)
+        t2_w = torch.softmax(t2, dim=0)                                                          # over the depth samples (eft.py:415)
+        f2 = (f2 * t2_w[..., None]).sum(dim=0)                                                   # [NC,N,256]
+        # ---- T3: sequence = input views, batch = rays
+        d3 = (2 if self.use_r else 1) * 78 + 256
+        d3p = (d3 + 3) // 4 * 4
+        tok3 = torch.zeros(NC, N, d3p, dtype=torch.float32, device=dev)
+        tok3[..., :78] = query_plucker[None]
+        o = 78
+        if self.use_r:
+            tok3[..., o:o + 78] = ref_plucker[:, :, D // 2, :]
+            o += 78
+        tok3[..., o:o + 256] = f2
+        f3 = self._transformer('t3', tok3.view(NC * N, d3p), NC, N).view(NC, N, 256)
+        t3_w = torch.softmax(torch.einsum('cnf,f->cn', f3, sd['t3_attn.weight'][0]) + sd['t3_attn.bias'], dim=0)   # over the views (eft.py:436)
+        f3 = (f3 * t3_w[..., None]).sum(dim=0)                                                   # [N,256]
+        rgb = f3 @ sd['color_layer.0.weight'].t() + sd['color_layer.0.bias']
+        if self.out_sigmoid:
+            rgb = torch.sigmoid(rgb)
+        return rgb, f3, t2_w, t3_w
 
     @torch.no_grad()
     def batched_forward(self, ray_bundle, n_batches: int = 32, return_intermediates=False, **kwargs):
@@ -350,3 +361,67 @@ class EpipolarFeatureTransformer(nn.Module):
         outs = [self.forward(RayBundle(o[i:i + 4096], d[i:i + 4096], l[i:i + 4096], None)) for i in range(0, o.shape[0], 4096)]
         a, b = (torch.cat([t[j] for t in outs], dim=0).view(*spatial, -1) for j in (0, 1))
         return a, b, 0
+
+    # ------------------------------------------------------------------------------------------------ view-batched feature cache
+    CACHE_RAYS = 4096       # rays (all depth samples, all input views) per transformer pass of feature_cache: the bound batched_forward keeps
+
+    @torch.no_grad()
+    def feature_cache(self, origins, directions, lengths, input_cameras, input_images, hw=None):
+        """the EFT feature cache of V query views at once (sparsefusion/distillation.py:95-125 without the per-view loop): what
+        ``batched_forward`` returns for each view v after ``encode(input_cameras[v], input_images)``, for all views in one pass.
+
+        origins / directions [V,N,3], lengths [V,N,D]: the query bundles; ``input_cameras``: the NC input cameras of every view in that view's
+        own frame -- one object whose R is [V,NC,3,3] (T [V,NC,3], focal_length / principal_point [V,NC,2]) or a sequence of V camera objects
+        with NC cameras each; ``input_images`` [NC,3,H,W] in [0,1], shared by every view.  ``hw`` = (h, w) with h * w = N (a square grid when
+        None).  Returns (features [V,256,h,w], rgb [V,3,h,w]): the conditioning features and the colour head's low-resolution image,
+        ``batched_forward``'s two outputs with return_features=True (utils/load_model.py:34) rearranged 'b h w f -> b f h w' (:110-118).
+
+        The ResNet-18 pyramid runs once (it depends on the images only; ``encode(None, input_images)``, which leaves ``input_cameras`` None).
+        Each T1 token row -- point, projection by its view's camera, look-ups, embeddings -- is written by one kernel (``sfb_eft_t1_tokens``);
+        the transformers run on whole views, at most ``CACHE_RAYS`` rays per pass (batched_forward's chunk), so the activations are bounded
+        whatever V is: building a scene's 82-view cache peaked at 2.7 GB (NC = 2) and 7.3 GB (NC = 6) of device memory on an H100
+        (tools/scene_bench.py)."""
+        if isinstance(input_cameras, (list, tuple)):
+            R = torch.stack([c.R for c in input_cameras])
+            T = torch.stack([c.T for c in input_cameras])
+            f = torch.stack([c.focal_length for c in input_cameras])
+            p = torch.stack([c.principal_point for c in input_cameras])
+        else:
+            R, T, f, p = input_cameras.R, input_cameras.T, input_cameras.focal_length, input_cameras.principal_point
+        V, N, D = lengths.shape
+        NC = R.shape[1]
+        if R.shape[0] != V or origins.shape[:2] != (V, N) or directions.shape[:2] != (V, N):
+            raise ValueError(f'feature_cache: {R.shape[0]} camera sets for bundles of {tuple(origins.shape[:2])} / {tuple(lengths.shape)}')
+        if hw is None:
+            s = math.isqrt(N)
+            if s * s != N:
+                raise ValueError(f'feature_cache: {N} rays per view is not a square grid; pass hw')
+            hw = (s, s)
+        self.encode(None, input_images)
+        if NC != self.encoder_latent.shape[0]:
+            raise ValueError(f'feature_cache: {NC} cameras per view for {self.encoder_latent.shape[0]} input images')
+        dev = self.encoder_latent.device
+        cams = torch.cat((R.reshape(V, NC, 9), T.reshape(V, NC, 3), f.reshape(V, NC, 2), p.reshape(V, NC, 2)), dim=-1).to(dev, torch.float32).contiguous()
+        origins, directions = origins.to(dev, torch.float32).contiguous(), directions.to(dev, torch.float32).contiguous()
+        lengths = lengths.to(dev, torch.float32).contiguous()
+        lat, img = self.encoder_latent, self._images_nhwc
+        d1p = (78 + 13 + self.feat_size + self.in_dim + 3) // 4 * 4
+        feats = torch.empty(V, 256, N, dtype=torch.float32, device=dev)
+        rgbs = torch.empty(V, 3, N, dtype=torch.float32, device=dev)
+        step = max(1, self.CACHE_RAYS // N)
+        with torch.cuda.device(dev):
+            for v0 in range(0, V, step):
+                v1 = min(V, v0 + step)
+                Vc = v1 - v0
+                M = Vc * N * D
+                tok1 = torch.empty(NC, M, d1p, dtype=torch.float32, device=dev)
+                lib.call('sfb_eft_t1_tokens', lib.fptr(cams[v0:v1]), lib.fptr(origins[v0:v1]), lib.fptr(directions[v0:v1]), lib.fptr(lengths[v0:v1]),
+                         lat.data_ptr(), lat.stride(2), lat.shape[1], lat.shape[2], self.feat_size, img.data_ptr(), img.stride(2), img.shape[1],
+                         img.shape[2], self.in_dim, float(self.omega0), lib.fptr(tok1), d1p, Vc, NC, N, D, lib.stream())
+                o, d = origins[v0:v1].reshape(Vc * N, 3), directions[v0:v1].reshape(Vc * N, 3)
+                query_plucker = self.encode_plucker(o, torch.nn.functional.normalize(d, dim=-1))             # [Vc*N, 78]
+                f1 = self._transformer('t1', tok1.view(NC * M, d1p), NC, M)
+                rgb, f3, _, _ = self._heads(tok1, f1, query_plucker, NC, Vc * N, D)
+                feats[v0:v1] = f3.view(Vc, N, 256).transpose(1, 2)
+                rgbs[v0:v1] = rgb.view(Vc, N, 3).transpose(1, 2)
+        return feats.view(V, 256, *hw), rgbs.view(V, 3, *hw)
