@@ -482,6 +482,33 @@ uint64_t sfb_palette_work_bytes(int B, int H, int W);
 int sfb_palette_quantize(const uint8_t* rgb, int B, int H, int W, int colors, uint8_t* palette, int32_t* ncolors, uint8_t* indices, void* work,
                          void* stream);
 
+/* ==========================================================================================
+ * section 12 -- albedo texture of an extracted mesh (NeRFRenderer.export_mesh(texture_size=T); the reference's textured export,
+ *    external/nerf/renderer_df.py:166-306, is never called there and needs xatlas and nvdiffrast).  A T x T texture, texel (x, y) = column x,
+ *    row y counted from the top; texel coordinates run over [0, T] with texel (x, y) covering [x, x+1) x [y, y+1).
+ * ========================================================================================== */
+/* Atlas of F triangles: n = ceil(sqrt(ceil(F / 2))) cells per row (1 when F = 0), cell size c = floor(T / n) texels.  Triangle t takes cell
+ * k = t / 2 at texel (x0, y0) = ((k % n) c, (k / n) c), half h = t % 2.  Its UV corners in tris[t, 0..2] order, in texels from (x0, y0),
+ * with m = 1/2 and d = 2:  h = 0: (m, m), (c-m-d, m), (m, c-m-d);  h = 1: (c-m, c-m), (m+d, c-m), (c-m, m+d).
+ * Ownership: texel (x0 + i, y0 + j), 0 <= i, j < c, belongs to triangle 2k when (2i+1) + (2j+1) < 2c and to 2k+1 otherwise, if that
+ * triangle exists; texels of unused cells and outside the n c square belong to none.  Every texel that a bilinear lookup at any point
+ * of a triangle's UV region weights nonzero belongs to that triangle.
+ * sfb_mesh_atlas_cell returns c, or 0 when c < SFB_TEXTURE_MIN_CELL or T is outside SFB_TEXTURE_MIN..SFB_TEXTURE_MAX (or F < 0). */
+#define SFB_TEXTURE_MIN 16
+#define SFB_TEXTURE_MAX 8192
+#define SFB_TEXTURE_MIN_CELL 4
+int sfb_mesh_atlas_cell(int F, int T);
+/* uv [F][3][2] fp32 <- the UV corners above in texel units, (x0 + u, y0 + v); exact (half-integers below 2^13). */
+int sfb_mesh_uv_atlas(int F, int T, float* uv, void* stream);
+/* Texels of rows [row0, row0 + rows), row-major: owner [rows*T] int32 (-1 = none) and xyz [rows*T][3] fp32 (0 where there is no owner).
+ * For an owned texel, p is the point of the owner's UV triangle closest to the texel centre (x + 1/2, y + 1/2) (the centre itself when
+ * inside), lambda its barycentrics, and xyz = sum_i lambda_i verts[tris[t, i]].  verts [V][3] fp32 (world units), tris [F][3] int32 with
+ * every index in 0..V-1 (not checked here); both may be NULL when F = 0. */
+int sfb_mesh_texel_points(const float* verts, const int32_t* tris, int F, int T, int row0, int rows, int32_t* owner, float* xyz, void* stream);
+/* out [n][3] uint8 <- trunc(255 rgb) where owner >= 0 (the reference's (feats * 255).astype(np.uint8)), 0 elsewhere.  rgb [n][3] fp32 in
+ * [0, 1], as sfb_ngp_field_forward writes it. */
+int sfb_mesh_texture_pack(const int32_t* owner, const float* rgb, int64_t n, uint8_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

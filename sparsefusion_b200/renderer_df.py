@@ -6,7 +6,8 @@ Same class / method names and keyword arguments (``render``, ``render_batched``,
 (``aabb_train``, ``aabb_infer``, and ``density_grid`` / ``density_bitfield`` / ``step_counter`` with cuda_ray), so
 ``ngp_network.render(rays_o, rays_d, staged=False, perturb=True, bg_color=0, ..., **vars(opt))`` works unchanged.
 ``export_mesh`` runs the reference's mcubes export on the GPU (sparsefusion_b200/mesh.py: lattice query through the fused field kernel,
-Gaussian smoothing, marching cubes, OBJ); the textured xatlas/nvdiffrast export, dead code in the reference, is not provided.
+Gaussian smoothing, marching cubes, OBJ); with ``texture_size`` it also bakes the field's albedo into a per-triangle UV atlas and writes a
+textured OBJ (the reference's xatlas/nvdiffrast export is dead code there).
 
 Every shading of the reference runs on both paths: 'albedo' (SparseFusion's) on the fused path below; 'lambertian' (any other
 string), 'textureless' and 'normal' shade the field with finite-difference normals computed as stencils inside the tiled field
@@ -200,22 +201,31 @@ class NeRFRenderer(nn.Module):
         self.local_step = 0
 
     @torch.no_grad()
-    def export_mesh(self, path, resolution=None, S=128, *, grid_resolution=128):
+    def export_mesh(self, path, resolution=None, S=128, *, grid_resolution=128, texture_size=None):
         """renderer_df.py:121-153 on the GPU: sigma on the lattice linspace(-bound, bound, R)^3 (indexing 'ij', queried in slabs of S
         x-planes), Gaussian smoothing with sigma = 1.5 voxels, marching cubes at mean + 0.25 std of the smoothed volume, and
         ``{path}/mcubes_mesh.obj`` with vertices in lattice index units, as the reference writes it.  ``resolution`` is accepted and
         ignored (the reference overrides it with 128); ``grid_resolution`` sets R (128 = the reference's lattice).
+        ``texture_size=T`` (16..8192) also writes ``{path}/mesh.obj`` (world-unit vertices with per-corner UVs), ``mesh.mtl`` and a T x T
+        ``albedo.png``: the field's albedo at the surface point under every texel of a per-triangle atlas (mesh.bake_albedo).  A T outside
+        16..8192 raises ValueError before anything is written; one too small for the mesh's triangle count raises it after mcubes_mesh.obj.
         Returns (verts [V,3] float32 in world units, v / (R-1) * 2 bound - bound; tris [F,3] int32) on the parameters' device.
         Works with either cuda_ray setting: it reads neither mean_density nor the density bitfield."""
         import os
         from . import mesh
         R = int(grid_resolution)
+        if texture_size is not None:
+            mesh._atlas_cell(0, texture_size)
         sigma = mesh.density_lattice(self, R, S)
         smooth = mesh.smooth_gaussian(sigma, 1.5)
         mean, std = mesh.volume_mean_std(smooth)
         verts, tris = mesh.marching_cubes(smooth, mean + 0.25 * std)
         mesh.write_obj(os.path.join(path, 'mcubes_mesh.obj'), verts, tris)
-        return verts / (R - 1) * (2 * self.bound) - self.bound, tris
+        verts_world = verts / (R - 1) * (2 * self.bound) - self.bound
+        if texture_size is not None:
+            uv, texture, _ = mesh.bake_albedo(self, verts_world, tris, texture_size)
+            mesh.write_textured_obj(path, verts_world, tris, uv, texture)
+        return verts_world, tris
 
     # ------------------------------------------------------------------------------------------ default path
     def run(self, rays_o, rays_d, num_steps=128, upsample_steps=128, light_d=None, ambient_ratio=1.0, shading='albedo', bg_color=None,

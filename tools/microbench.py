@@ -334,7 +334,8 @@ def sample_bench(out):
 def mesh_bench(out):
     """NeRFRenderer.export_mesh stage by stage at R = 128, 256, 512 (seeded field, +-0.5 embeddings): device-event times of the lattice
     query, smoothing, statistics (includes the host read of the two doubles), marching-cubes count (includes the host read of V and F) and
-    emit, medians of 5 after one warm-up; the host OBJ write is timed separately (wall clock, to a temporary directory)."""
+    emit, medians of 5 after one warm-up; the host OBJ write is timed separately (wall clock, to a temporary directory).  Each mesh is then
+    textured at T = 2048 (texture_stages)."""
     import subprocess
     import tempfile
     import time
@@ -383,16 +384,62 @@ def mesh_bench(out):
                     mesh.write_obj(os.path.join(d, 'mcubes_mesh.obj'), verts, tris)
                     t_w = (time.perf_counter() - t0) * 1e3
                     obj_mb = os.path.getsize(os.path.join(d, 'mcubes_mesh.obj')) / 1e6
+                tex_t = texture_stages(net, verts / (R - 1) * (2 * net.bound) - net.bound, tris, ev)
                 if it:
-                    rows.append((t_q, t_s, t_st, t_c, t_e, t_w))
+                    rows.append((t_q, t_s, t_st, t_c, t_e, t_w) + tex_t)
                 del sig, sm, scratch
             med = [float(m) for m in np.median(np.array(rows), axis=0)]
             gpu = sum(med[:5])
             rec = dict(field_query_ms=round(med[0], 2), smooth_ms=round(med[1], 2), stats_ms=round(med[2], 2), mc_count_ms=round(med[3], 2),
                        mc_emit_ms=round(med[4], 2), gpu_total_ms=round(gpu, 2), obj_write_ms=round(med[5], 1), vertices=nv, triangles=nf,
                        obj_mb=round(obj_mb, 1), gpu_share=round(gpu / (gpu + med[5]), 3))
+            tex_gpu = sum(med[6:10])
+            rec['texture'] = dict(T=TEX_T, uv_atlas_ms=round(med[6], 3), texel_points_ms=round(med[7], 3), field_query_ms=round(med[8], 2),
+                                  pack_ms=round(med[9], 3), gpu_total_ms=round(tex_gpu, 2), bake_albedo_ms=round(med[10], 2),
+                                  write_textured_obj_ms=round(med[11], 1), png_of_it_ms=round(med[12], 1), cell=_lib.load().sfb_mesh_atlas_cell(nf, TEX_T))
             out['mesh'][str(R)] = rec
             print('mesh', R, rec, flush=True)
+
+
+TEX_T = 2048
+
+
+def texture_stages(net, verts_world, tris, ev):
+    """the texture stages of export_mesh(texture_size=2048) on one mesh: uv atlas, texel points, field query and pack over the whole texture
+    in one launch each (bake_albedo runs the last three per slab of 1024 rows), bake_albedo end to end, all as device events; then the
+    host write_textured_obj (mesh.obj, mesh.mtl, albedo.png) and, apart, the albedo.png save alone (Pillow), by wall clock, to a temporary
+    directory"""
+    import tempfile
+    import time
+    from sparsefusion_b200 import _lib, mesh
+    T, F = TEX_T, tris.shape[0]
+    f = _lib.fptr
+    emb, w0, b0, w1, b1, w2, b2 = net._field_params()
+    enc = net.encoder
+    geo = (float(np.log2(enc.per_level_scale)), int(enc.base_resolution), float(net.bound))
+    uv = torch.empty(F, 3, 2, device='cuda')
+    owner = torch.empty(T * T, dtype=torch.int32, device='cuda')
+    xyz, rgb = torch.empty(T * T, 3, device='cuda'), torch.empty(T * T, 3, device='cuda')
+    sigma, tex = torch.empty(T * T, device='cuda'), torch.empty(T, T, 3, dtype=torch.uint8, device='cuda')
+    st = _lib.stream()
+    _, t_uv = ev(lambda: _lib.call('sfb_mesh_uv_atlas', F, T, uv.data_ptr(), st))
+    _, t_pts = ev(lambda: _lib.call('sfb_mesh_texel_points', f(verts_world.contiguous()), _lib.iptr(tris), F, T, 0, T, owner.data_ptr(),
+                                    xyz.data_ptr(), st))
+    _, t_q = ev(lambda: _lib.call('sfb_ngp_field_forward', f(xyz), None, None, None, 0, T * T, f(emb), _lib.iptr(enc.offsets), *geo, f(w0),
+                                  f(b0), f(w1), f(b1), f(w2), f(b2), f(sigma), f(rgb), st))
+    _, t_pack = ev(lambda: _lib.call('sfb_mesh_texture_pack', owner.data_ptr(), rgb.data_ptr(), T * T, tex.data_ptr(), st))
+    (uv2, tex2, _), t_bake = ev(lambda: mesh.bake_albedo(net, verts_world, tris, T))
+    assert torch.equal(tex2, tex) and torch.equal(uv2, uv)
+    with tempfile.TemporaryDirectory() as d:
+        from PIL import Image
+        img = tex2.cpu().numpy()
+        t0 = time.perf_counter()
+        mesh.write_textured_obj(d, verts_world, tris, uv2, tex2)
+        t_all = (time.perf_counter() - t0) * 1e3
+        t0 = time.perf_counter()
+        Image.fromarray(img, 'RGB').save(os.path.join(d, 'albedo.png'))
+        t_png = (time.perf_counter() - t0) * 1e3
+    return t_uv, t_pts, t_q, t_pack, t_bake, t_all, t_png
 
 
 def scenes_bench(out):
