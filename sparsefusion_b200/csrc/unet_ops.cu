@@ -1171,7 +1171,9 @@ int sfb_groupnorm_nhwc(const float* x, int64_t ldx, int NB, int HW, int C, int G
             return check_launch("groupnorm_nhwc(cluster)");
         }
     }
-    const bool rows_ok = (Cg % 4 == 0) && (C4 <= 256 ? (256 % C4 == 0) : (C4 % 256 == 0)) && (Cg / 4 <= (C4 < 256 ? C4 : 256));
+    // gn_stats_rows_kernel hands each 256-column pass cols / Cg4 whole groups: a group that straddles two passes would mix two groups' columns
+    // and leave the last groups' partials unwritten (C = 3072 or 5120 with 8 groups), so such shapes take the group-major kernel
+    const bool rows_ok = (Cg % 4 == 0) && (C4 <= 256 ? (256 % C4 == 0) : (C4 % 256 == 0 && 256 % (Cg / 4) == 0));
     int S = 1;
     if (rows_ok) {
         const int rpi = 256 / (C4 < 256 ? C4 : 256);
