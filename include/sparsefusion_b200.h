@@ -249,6 +249,13 @@ int sfb_plms_update(const float* x, const float* e0, const float* e1, const floa
 int sfb_plms_update_rows(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1, float c2,
                          float c3, const float* noise, const float* row_scalars, float clip, float* x_prev, float* x0_out,
                          int rows, int64_t row_len, void* stream);
+/* sfb_plms_update_rows with classifier-free guidance (PLMSSampler.sample with cond_scale != 1): the step's new eps is
+ *   e_t = e_null + (e_cond - e_null) * cond_scale   (imagen_pytorch.py:572-577, rounded without contraction)
+ * and takes e0's place in e' = c0*e_t + c1*e1 + c2*e2 + c3*e3.  e_out (may be NULL) receives e_t, the eps the sampler keeps in its history.
+ * e_cond / e_null hold `rows` contiguous rows each (the conditional and null halves of one batch-2*rows UNet evaluation). */
+int sfb_plms_update_rows_cfg(const float* x, const float* e_cond, const float* e_null, float cond_scale, const float* e1, const float* e2,
+                             const float* e3, float c0, float c1, float c2, float c3, const float* noise, const float* row_scalars, float clip,
+                             float* x_prev, float* e_out, int rows, int64_t row_len, void* stream);
 
 /* One step of DDPM.p_sample with dynamic thresholding (sparsefusion/vldm.py:289-361), B rows of row_len floats (row_len <= 65536):
  *   e = cond_scale*e_cond + (1-cond_scale)*e_null (e_null may be NULL: e = e_cond);  x0 = (x - sigma*e) / max(alpha,1e-8);

@@ -1354,12 +1354,13 @@ int sfb_gate_residual_nhwc(const float* h, int64_t ldh, const float* gate, const
 // plms_update_rows_kernel is the same element for a batch whose rows sit at different noise levels (scene-batched sampling): row blockIdx.y reads
 // its five scalars from a table.  Both kernels run plms_update_element, so a row's result is bit-identical to a separate sfb_plms_update launch.
 namespace sfb {
-__device__ __forceinline__ void plms_update_element(int64_t i, const float* __restrict__ x, const float* __restrict__ e0,
-                                                    const float* __restrict__ e1, const float* __restrict__ e2, const float* __restrict__ e3,
-                                                    float c0, float c1, float c2, float c3, const float* __restrict__ noise, float alpha,
-                                                    float sigma, float alpha_next, float c, float noise_scale, float clip,
-                                                    float* __restrict__ x_prev, float* __restrict__ x0_out, float* __restrict__ e_out) {
-    float e = c0 * e0[i];
+// element i with e0's value already loaded (e0v)
+__device__ __forceinline__ void plms_update_value(int64_t i, float e0v, const float* __restrict__ x, const float* __restrict__ e1,
+                                                  const float* __restrict__ e2, const float* __restrict__ e3, float c0, float c1, float c2,
+                                                  float c3, const float* __restrict__ noise, float alpha, float sigma, float alpha_next, float c,
+                                                  float noise_scale, float clip, float* __restrict__ x_prev, float* __restrict__ x0_out,
+                                                  float* __restrict__ e_out) {
+    float e = c0 * e0v;
     if (e1) e += c1 * e1[i];
     if (e2) e += c2 * e2[i];
     if (e3) e += c3 * e3[i];
@@ -1370,6 +1371,14 @@ __device__ __forceinline__ void plms_update_element(int64_t i, const float* __re
     x_prev[i] = mean + noise_scale * noise[i];
     if (x0_out) x0_out[i] = x0;
     if (e_out) e_out[i] = e;
+}
+
+__device__ __forceinline__ void plms_update_element(int64_t i, const float* __restrict__ x, const float* __restrict__ e0,
+                                                    const float* __restrict__ e1, const float* __restrict__ e2, const float* __restrict__ e3,
+                                                    float c0, float c1, float c2, float c3, const float* __restrict__ noise, float alpha,
+                                                    float sigma, float alpha_next, float c, float noise_scale, float clip,
+                                                    float* __restrict__ x_prev, float* __restrict__ x0_out, float* __restrict__ e_out) {
+    plms_update_value(i, e0[i], x, e1, e2, e3, c0, c1, c2, c3, noise, alpha, sigma, alpha_next, c, noise_scale, clip, x_prev, x0_out, e_out);
 }
 
 __global__ void plms_update_kernel(const float* __restrict__ x, const float* __restrict__ e0, const float* __restrict__ e1,
@@ -1400,6 +1409,32 @@ __global__ void plms_update_rows_kernel(const float* __restrict__ x, const float
         plms_update_element(i, x + off, e0 + off, r1, r2, r3, c0, c1, c2, c3, noise + off, alpha, sigma, alpha_next, c, noise_scale, clip,
                             x_prev + off, rx0, nullptr);
 }
+
+// Classifier-free guidance in front of the same element: e_t = e_null + (e_cond - e_null) * cond_scale (imagen_pytorch.py:572-577) is formed
+// in a register, written to e_out (the sampler's eps history holds the guided eps, as the reference's p_sample returns it) and takes e0's place
+// in the combination, so the update rounds exactly as plms_update_rows_kernel with e0 = e_out.
+__global__ void plms_update_rows_cfg_kernel(const float* __restrict__ x, const float* __restrict__ e_cond, const float* __restrict__ e_null,
+                                            float cond_scale, const float* __restrict__ e1, const float* __restrict__ e2,
+                                            const float* __restrict__ e3, float c0, float c1, float c2, float c3, const float* __restrict__ noise,
+                                            const float* __restrict__ row_scalars, float clip, float* __restrict__ x_prev,
+                                            float* __restrict__ e_out, int64_t row_len) {
+    pdl_sync();
+    __shared__ float s[5];
+    const int64_t off = (int64_t)blockIdx.y * row_len;
+    if (threadIdx.x < 5) s[threadIdx.x] = row_scalars[blockIdx.y * 5 + threadIdx.x];
+    __syncthreads();
+    const float alpha = s[0], sigma = s[1], alpha_next = s[2], c = s[3], noise_scale = s[4];
+    const float* r1 = e1 ? e1 + off : nullptr;
+    const float* r2 = e2 ? e2 + off : nullptr;
+    const float* r3 = e3 ? e3 + off : nullptr;
+    for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < row_len; i += (int64_t)gridDim.x * blockDim.x) {
+        const float en = e_null[off + i];
+        const float et = __fadd_rn(en, __fmul_rn(__fsub_rn(e_cond[off + i], en), cond_scale));   // no FMA contraction: the reference's rounding
+        if (e_out) e_out[off + i] = et;
+        plms_update_value(i, et, x + off, r1, r2, r3, c0, c1, c2, c3, noise + off, alpha, sigma, alpha_next, c, noise_scale, clip, x_prev + off,
+                          nullptr, nullptr);
+    }
+}
 }  // namespace sfb
 
 extern "C" int sfb_plms_update(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1, float c2,
@@ -1425,6 +1460,19 @@ extern "C" int sfb_plms_update_rows(const float* x, const float* e0, const float
     SFB_LAUNCH(sfb::plms_update_rows_kernel, dim3((unsigned)bx, (unsigned)rows), 256, 0, sfb::as_stream(stream), x, e0, e1, e2, e3, c0, c1, c2, c3,
                noise, row_scalars, clip, x_prev, x0_out, row_len);
     return sfb::check_launch("plms_update_rows");
+}
+
+extern "C" int sfb_plms_update_rows_cfg(const float* x, const float* e_cond, const float* e_null, float cond_scale, const float* e1, const float* e2,
+                                        const float* e3, float c0, float c1, float c2, float c3, const float* noise, const float* row_scalars,
+                                        float clip, float* x_prev, float* e_out, int rows, int64_t row_len, void* stream) {
+    if (rows == 0 || row_len == 0) return SFB_OK;
+    SFB_REQUIRE(x && e_cond && e_null && noise && row_scalars && x_prev, "plms_update_rows_cfg: null pointer");
+    SFB_REQUIRE(rows > 0 && rows <= 65535 && row_len > 0, "plms_update_rows_cfg: rows must be in [1, 65535]");
+    int64_t bx = (row_len + 255) / 256;
+    if (bx > 1024) bx = 1024;
+    SFB_LAUNCH(sfb::plms_update_rows_cfg_kernel, dim3((unsigned)bx, (unsigned)rows), 256, 0, sfb::as_stream(stream), x, e_cond, e_null, cond_scale,
+               e1, e2, e3, c0, c1, c2, c3, noise, row_scalars, clip, x_prev, e_out, row_len);
+    return sfb::check_launch("plms_update_rows_cfg");
 }
 
 // ------------------------------------------------------------------------------------ DDPM ancestral step with dynamic thresholding

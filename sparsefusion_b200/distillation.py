@@ -75,7 +75,8 @@ def shard_views(views: list, rank: int, world_size: int) -> list:
 
 def view_seed(seed: int, itr: int, view: int, stream: int) -> int:
     """seed of the generator that serves ONE (iteration, view, stream) -- stream 0: photometric render, 1: fusion render, 2: PLMS noise, 3: evaluation
-    render (``evaluate.evaluate_scene``, with iteration 0), 4: circle-path render (``evaluate.render_views`` for the fly-around gif, iteration 0).
+    render (``evaluate.evaluate_scene``, with iteration 0), 4: circle-path render (``evaluate.render_views`` for the fly-around gif, iteration 0), 5: VLDM
+    baseline samples (``baselines.sample_vldm_views``, iteration 0).
     Keyed draws make a minibatch step independent of how its views are spread over ranks."""
     x = (seed * 0x9E3779B97F4A7C15 + itr * 0xBF58476D1CE4E5B9 + view * 0x94D049BB133111EB + stream * 0xD6E8FEB86659FD93) & 0xFFFFFFFFFFFFFFFF
     x ^= x >> 31
@@ -738,7 +739,7 @@ class NativeSceneBuilder:
 
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
-                      process_group=None, evaluate=False, visualize=False, visualize_shadings=()):
+                      process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -766,6 +767,11 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ``loss_fn_vgg`` unless ``evaluate``.  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
     torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``, ``visualize``,
     ``visualize_shadings``.
+
+    ``evaluate_baselines=True`` (needs ``use_diffusion`` and the builder's ``eval_views``) also scores the paper's two intermediate stages on
+    the scene views after the loop (``baselines.evaluate_baselines``): the cached EFT images and VLDM samples from pure noise conditioned on
+    the cached EFT features (guidance scale ``vldm_cond_scale``, draws keyed by the scene's seed), with the same metrics as ``evaluate``, and
+    writes ``{save_dir}/metrics/{seq_name}_eft.txt``, ``{seq_name}_vldm.txt`` and ``{save_dir}/render_gifs/{seq_name}_baselines.gif``.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     rank, world = 0, 1
@@ -778,13 +784,13 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
                          start_percep_step=1000, views_per_step=views_per_step)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
-                                     visualize_shadings)
+                                     visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
-                   evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=()):
+                   evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -794,7 +800,8 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     ``on_iteration(itr, multi_scene_distiller)`` runs after every iteration.  ``evaluate`` / ``loss_fn_vgg``: each scene is scored and its
     ``{save_dir}/metrics/{seq_name}.txt`` written as ``distillation_loop(evaluate=True)`` does, scene k's render jitter keyed by ``seed + k``.
     ``visualize`` / ``visualize_shadings``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter
-    keyed by ``seed + k``.
+    keyed by ``seed + k``.  ``evaluate_baselines`` / ``vldm_cond_scale``: each scene's EFT and VLDM baselines scored and written as
+    ``distillation_loop(evaluate_baselines=True)`` does, scene k's VLDM draws keyed by ``seed + k``.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
 
@@ -803,7 +810,12 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
-                             loss_fn_vgg, visualize, visualize_shadings)
+                             loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
+
+
+def _baselines(enabled, vae, vldm, cond_scale):
+    """what ``_run_distillation`` needs to score the EFT / VLDM baselines, or None when they are off"""
+    return dict(vae=vae, vldm=vldm, cond_scale=float(cond_scale)) if enabled else None
 
 
 EFT_GRID_COLUMNS = 8     # cached EFT images per row of the grid the reference writes before its loop (:129-141)
@@ -860,11 +872,12 @@ def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_image
 
 
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
-                      loss_fn_vgg=None, visualize=False, visualize_shadings=()):
+                      loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
     ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
-    grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``).  Returns the networks."""
+    grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``); with ``baselines`` (``_baselines``), the EFT and VLDM
+    scores, metrics files and gifs after it.  Returns the networks."""
     import os
     from .lpips_vgg import PerceptualLoss
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
@@ -874,9 +887,14 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     if visualize:
         from .video import require_pillow
         require_pillow()
-    for flag, name, sig in ((evaluate or visualize, 'eval_views', '(scene_cameras, scene_rgb, scene_mask)'), (visualize, 'circle_views', '(scene_cameras)')):
+    if baselines is not None:
+        from .baselines import check_baseline_options
+        check_baseline_options(baselines['vldm'], baselines['cond_scale'], use_diffusion)
+        from .video import require_pillow
+        require_pillow()
+    for flag, name, sig in ((evaluate or visualize or baselines is not None, 'eval_views', '(scene_cameras, scene_rgb, scene_mask)'), (visualize, 'circle_views', '(scene_cameras)')):
         if flag and not callable(getattr(builder, name, None)):
-            raise TypeError(f'{"evaluate=True" if name == "eval_views" and evaluate else "visualize=True"} needs the scene builder to provide '
+            raise TypeError(f'{_needs(name, evaluate, visualize)} needs the scene builder to provide '
                             f'{name}{sig}; {type(builder).__name__} has none')
     exp_dir = getattr(args, 'exp_dir', save_dir)
     for sc in scenes:
@@ -884,10 +902,14 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
     os.makedirs(save_dir, exist_ok=True)
     device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
-    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate or visualize else None
+    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate or visualize or baselines else None
     circles = [tuple(t.to(device) for t in builder.circle_views(cams)) for _, cams, _, _, _, _ in scenes] if visualize else None
     caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
               for _, cams, rgb, mask, _, input_idx in scenes]
+    if baselines is not None:
+        from .baselines import check_baseline_cache
+        for views, cache in zip(eval_views, caches):
+            check_baseline_cache(cache, views)
     if visualize and use_diffusion:
         for (seq_name, *_rest), views, cache in zip(scenes, eval_views, caches):
             need = -(-views.rgb.shape[0] // EFT_GRID_COLUMNS) * EFT_GRID_COLUMNS
@@ -912,10 +934,10 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
         torch.cuda.synchronize(device)
     for (seq_name, *_rest), ngp in zip(scenes, ngps):
         torch.save({'model_state_dict': ngp.state_dict()}, f'{save_dir}/{seq_name}.pt')                             # :495-496
-    if evaluate or visualize:
+    if evaluate or visualize or baselines is not None:
         from .evaluate import evaluate_scene, write_scene_metrics
         with torch.cuda.device(device):
-            eval_percep = None if loss_fn_vgg is None or not evaluate else PerceptualLoss('vgg', device=device).load_state_dict(loss_fn_vgg.state_dict())
+            eval_percep = None if loss_fn_vgg is None or not (evaluate or baselines) else PerceptualLoss('vgg', device=device).load_state_dict(loss_fn_vgg.state_dict())
             for k, ((seq_name, *_rest), ngp, views) in enumerate(zip(scenes, ngps, eval_views)):
                 scores = None
                 if evaluate:
@@ -926,4 +948,17 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
                 if visualize:
                     _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circles[k], caches[k].target_eft_image if use_diffusion else None,
                                           base_seed + k, scores, visualize_shadings)                                # :444-493
+            if baselines is not None:
+                from .baselines import evaluate_baselines
+                sampler = PLMSSampler(baselines['vldm'], 50)                                                        # plms_steps of the loop (:160)
+                for k, ((seq_name, *_rest), views) in enumerate(zip(scenes, eval_views)):
+                    evaluate_baselines(save_dir, seq_name, baselines['vldm'], baselines['vae'], caches[k], views, eval_percep, seed=base_seed + k,
+                                       cond_scale=baselines['cond_scale'], sampler=sampler)
     return ngps
+
+
+def _needs(name, evaluate, visualize):
+    """the option that asked the scene builder for ``name``, for the error message"""
+    if name == 'eval_views':
+        return 'evaluate=True' if evaluate else 'visualize=True' if visualize else 'evaluate_baselines=True'
+    return 'visualize=True'

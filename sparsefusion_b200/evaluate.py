@@ -40,7 +40,7 @@ class SceneEval:
     ssim: torch.Tensor        # [V]  fp32 values, as scikit-image returns them for fp32 images
     lpips: torch.Tensor       # [V]  nan without a perceptual network
     image: torch.Tensor       # [V, H, W, 3]
-    silhouette: torch.Tensor  # [V, H, W]  weights_sum
+    silhouette: torch.Tensor  # [V, H, W]  weights_sum; None for the baselines (baselines.evaluate_baselines), which render nothing
 
 
 def image_metrics(pred: torch.Tensor, gt: torch.Tensor):
@@ -117,15 +117,25 @@ def evaluate_scene(ngp, views: EvalViews, opt, percep, *, seed: int) -> SceneEva
     if N != H * W or views.rgb.shape[:2] != (V, 3) or views.rays_d.shape != views.rays_o.shape:
         raise ValueError(f'evaluate_scene: rays {tuple(views.rays_o.shape)} / {tuple(views.rays_d.shape)} do not match images {tuple(views.rgb.shape)}')
     image, sil = render_views(ngp, views.rays_o, views.rays_d, (H, W), opt, seed=seed, stream=EVAL_STREAM)
+    return score_images(image, views.rgb, percep, silhouette=sil)
+
+
+@torch.no_grad()
+def score_images(image: torch.Tensor, rgb: torch.Tensor, percep, silhouette=None) -> SceneEval:
+    """``evaluate_scene``'s scores of images [V, H, W, 3] (fp32 CUDA) against the ground truth ``rgb`` [V, 3, H, W]: SSIM / PSNR by
+    ``image_metrics`` over all views at once, LPIPS by ``percep.value_and_grad(image, gt, normalize=True, want_grad=False)`` per view (nan
+    when ``percep`` is None)"""
+    dev = image.device
+    V = image.shape[0]
     with torch.cuda.device(dev):
-        gt = views.rgb.float().permute(0, 2, 3, 1).contiguous()
+        gt = rgb.float().permute(0, 2, 3, 1).contiguous()
         ssim, psnr = image_metrics(image, gt)
         if percep is None:
             lp = torch.full((V,), float('nan'), dtype=torch.float64, device=dev)
         else:
-            lp = torch.stack([percep.value_and_grad(image[v].permute(2, 0, 1), views.rgb[v].float(), normalize=True, want_grad=False)[0]
+            lp = torch.stack([percep.value_and_grad(image[v].permute(2, 0, 1), rgb[v].float(), normalize=True, want_grad=False)[0]
                               for v in range(V)]).double()
-    return SceneEval(psnr=psnr, ssim=ssim, lpips=lp, image=image, silhouette=sil)
+    return SceneEval(psnr=psnr, ssim=ssim, lpips=lp, image=image, silhouette=silhouette)
 
 
 def _array(values) -> np.ndarray:

@@ -12,7 +12,9 @@ combination, x0 prediction + clamp, posterior mean, noise injection: ~30 eager l
 kernel (``sfb_plms_update``).  Every ``torch.randn_like`` of the reference is routed through ``self.noise_fn`` (default
 ``torch.randn_like``) in the reference's draw order and count (including the draws whose result the reference discards), so
 parity tests can inject the oracle's noise (SURVEY.md Appendix C).  ``p_sample`` / ``get_model_output`` remain as the
-reference-shaped (unfused) methods; ``plms_sample_loop`` uses the fused path on CUDA.
+reference-shaped (unfused) methods; ``plms_sample_loop`` uses the fused path on CUDA.  With classifier-free guidance (``cond_scale != 1``)
+each evaluation is ONE batch-2B graph replay of the conditional and null rows, and the guided eps is formed inside the update kernel
+(``sfb_plms_update_rows_cfg``), as ``DDPM.sample`` does it.
 
 ``sample_rows`` runs a batch whose rows each have their own ``max_thres`` (scene-batched distillation): the rows share every round of UNet
 evaluation while they are still running (``RowSchedule``), and the update kernel takes its scalars per row (``sfb_plms_update_rows``).  The same
@@ -138,16 +140,29 @@ class PLMSSampler:
     def _eps(self, unet, x, log_snr, cond_images, cond_scale, time_features=None):
         self.last_unet_calls += 1
         if self.use_cuda_graph and cond_scale == 1:
-            if self._graph is None or self._graph.unet is not unet:
-                self._graph = UnetGraph(unet)
-            # cond_images is fixed for the whole run (per batch size: a shrinking batch is a prefix of it): its share of init_conv is evaluated by
-            # the first call of each batch size only
-            b = x.shape[0]
-            new_cond = b not in self._cond_batches
-            self._cond_batches.add(b)
-            self.last_graph_replays += 1
-            return self._graph(x, log_snr, cond_images, new_cond=new_cond, time_features=time_features).clone()
+            return self._replay(unet, x, log_snr, cond_images, time_features).clone()
         return unet.forward_with_cond_scale(x, log_snr, cond_images=cond_images, cond_scale=cond_scale)
+
+    def _replay(self, unet, x, log_snr, cond_images, time_features):
+        """one evaluation replayed from the CUDA graph of x's batch size; returns the graph's static output"""
+        if self._graph is None or self._graph.unet is not unet:
+            self._graph = UnetGraph(unet)
+        # cond_images is fixed for the whole run (per batch size: a shrinking batch is a prefix of it): its share of init_conv is evaluated by
+        # the first call of each batch size only
+        b = x.shape[0]
+        new_cond = b not in self._cond_batches
+        self._cond_batches.add(b)
+        self.last_graph_replays += 1
+        return self._graph(x, log_snr, cond_images, new_cond=new_cond, time_features=time_features)
+
+    def _eps_pair(self, unet, x_pair, log_snr, cond_pair, time_features):
+        """the conditional and the null eps of a guided step as ONE UNet batch: ``x_pair`` = cat(x, x), ``cond_pair`` = cat(cond, cond * 0) (the
+        reference's cond_drop_prob = 1 branch zeroes the conditioning, imagen_pytorch.py:1467).  A graph replay -- its static output, which the
+        step's update kernel consumes before the next replay -- or, without CUDA graphs, one eager evaluation."""
+        self.last_unet_calls += 1
+        if self.use_cuda_graph:
+            return self._replay(unet, x_pair, log_snr, cond_pair, time_features)
+        return unet.forward(x_pair, log_snr, cond_images=cond_pair)
 
     def _start_run(self):
         self.last_unet_calls = 0
@@ -156,8 +171,14 @@ class PLMSSampler:
 
     @torch.no_grad()
     def sample(self, image=None, max_thres=.999, cond_images=None, cond_scale=1.0, use_tqdm=True, return_noise=False, **kwargs):
-        batch_size = cond_images.shape[0]
+        """``cond_scale != 1``: classifier-free guidance, eps = null + (cond - null) * cond_scale (external/plms.py:25,136-154); on CUDA the two
+        branches are one batch-2B UNet evaluation (``_eps_pair``) and the guided eps is formed inside the step's update kernel.  Refused
+        (ValueError) when the VLDM was built without conditional dropout (``cond_drop_prob == 0``), as ``DDPM.sample`` refuses it."""
         d = self.diffusion
+        if cond_scale != 1 and not d.can_classifier_guidance:
+            raise ValueError('PLMSSampler.sample: the VLDM was not trained with conditional dropout (cond_drop_prob == 0), so classifier-free '
+                             f'guidance (cond_scale {cond_scale} != 1) is not available')
+        batch_size = cond_images.shape[0]
         shape = (batch_size, d.sample_channels[0], d.image_sizes[0], d.image_sizes[0])
         img, x_noisy, noise, alpha_cumprod = self.plms_sample_loop(d.unets[0], image=image, shape=shape, cond_images=cond_images,
                                                                    cond_scale=cond_scale, noise_scheduler=d.noise_schedulers[0],
@@ -235,11 +256,16 @@ class PLMSSampler:
     def _fused_loop(self, unet, image, cond_images, cond_scale, max_thres):
         """plms_sample_loop (:54-119) + p_sample (:122-156) with the per-step latent math in one kernel.  ``max_thres`` is one float (every row
         runs the same schedule: ``sample``) or one float per row (``sample_rows``); see ``RowSchedule`` for how rows of different lengths share
-        the rounds."""
+        the rounds.  Guided (``cond_scale != 1``, one schedule only): each round evaluates the rows cat(x, x) with cat(cond, cond * 0) as one
+        UNet batch and ``sfb_plms_update_rows_cfg`` forms the guided eps in front of the Adams-Bashforth combination; the history keeps the
+        guided eps the kernel writes out, as the reference's p_sample returns it."""
         S = image.shape[0]
         dev = image.device
         clip = float(self.diffusion.clip_value)
         same = not isinstance(max_thres, (list, tuple))
+        guided = cond_scale != 1
+        if guided and not same:
+            raise NotImplementedError('PLMSSampler: classifier-free guidance runs with one schedule for every row (sample), not per-row schedules')
         mts = [float(max_thres)] * S if same else list(max_thres)
         same = same or len(set(mts)) == 1
         sch = row_schedule(mts, self.plms_steps)
@@ -282,12 +308,14 @@ class PLMSSampler:
             img = torch.where(hi_t > 0.5, image, x_noisy)
         cur = img if identity else img.index_select(0, perm_d)
         cond = cond_images if identity else cond_images.index_select(0, perm_d)
+        if guided:                                                                # the conditional rows, then the null rows (every round has S rows)
+            cond = torch.cat((cond, torch.zeros_like(cond))).contiguous()
         row_len = image[0].numel()
 
         # the run's noise levels are known now: everything of the UNet that depends on them only (time embedding, conditioning tokens, all
         # time MLPs) is evaluated for the whole run in one batch (Unet.precompute_time) instead of once per evaluation
         tf_all = None
-        if self.use_cuda_graph and cond_scale == 1 and R > 0 and hasattr(unet, 'precompute_time'):
+        if self.use_cuda_graph and R > 0 and hasattr(unet, 'precompute_time'):
             tf_all = unet.precompute_time(levels_ls)
 
         def draw(like, b):
@@ -296,14 +324,31 @@ class PLMSSampler:
             return self.noise_fn(like, rows=order[:b])
 
         def eps_at(x, j, b):
+            """the round's eps [b]; guided: the conditional and null eps [2b] of the round, for update_guided"""
             tf = None
+            nb = 2 * b if guided else b
             if tf_all is not None:
                 idx = sch.level_idx[j]
                 if len(set(idx)) == 1:
-                    tf = {k: v[idx[0]:idx[0] + 1].expand(b, *v.shape[1:]) for k, v in tf_all.items()}
+                    tf = {k: v[idx[0]:idx[0] + 1].expand(nb, *v.shape[1:]) for k, v in tf_all.items()}
                 else:
                     tf = {k: v.index_select(0, lvl_tab[j, :b]) for k, v in tf_all.items()}
+            if guided:
+                return self._eps_pair(unet, torch.cat((x, x)), ls_tab[j, :b].repeat(2) if tf is None else None, cond, tf)
             return self._eps(unet, x, ls_tab[j, :b], cond[:b], cond_scale, time_features=tf)
+
+        def update_guided(x, pair, hist, coefs, z, j, b, keep):
+            """update of round j whose new eps is the guided combination of ``pair``'s halves, weighted coefs[0]; ``hist`` / coefs[1:] the older
+            eps.  Returns (x_prev, guided eps, or None unless ``keep``)."""
+            out = torch.empty_like(x)
+            e_t = torch.empty_like(x) if keep else None
+            hist = [e[:b].contiguous() for e in hist]
+            z = z.contiguous()
+            ptrs = [lib.fptr(e) for e in hist] + [None] * (3 - len(hist))
+            cf = list(coefs) + [0.0] * (4 - len(coefs))
+            lib.call('sfb_plms_update_rows_cfg', lib.fptr(x), lib.fptr(pair[:b]), lib.fptr(pair[b:]), float(cond_scale), *ptrs, *cf, lib.fptr(z),
+                     lib.fptr(sc_tab[j, :b]), clip, lib.fptr(out), lib.fptr(e_t), b, row_len, st())
+            return out, e_t
 
         def update(x, eps_list, coefs, z, j, b):
             out = torch.empty_like(x)
@@ -324,7 +369,10 @@ class PLMSSampler:
             if j == 0:
                 e_t = eps_at(cur, 0, b)
                 draw(cur, b)                                                      # draw of the first get_model_output call (:136; result unused)
-                x_prev = update(cur, [e_t], [1.0], draw(cur, b), 0, b)            # pseudo improved Euler predictor (:137-143)
+                if guided:
+                    x_prev, e_t = update_guided(cur, e_t, [], [1.0], draw(cur, b), 0, b, True)
+                else:
+                    x_prev = update(cur, [e_t], [1.0], draw(cur, b), 0, b)        # pseudo improved Euler predictor (:137-143)
                 continue
             if j == 1:
                 e_next = eps_at(x_prev, 1, b)
@@ -339,7 +387,14 @@ class PLMSSampler:
                     eps_list, coefs = [e_t, old_eps[-1], old_eps[-2]], [23 / 12, -16 / 12, 5 / 12]
                 else:
                     eps_list, coefs = [e_t, old_eps[-1], old_eps[-2], old_eps[-3]], [55 / 24, -59 / 24, 37 / 24, -9 / 24]
-            cur = update(cur, eps_list, coefs, draw(cur, b), j, b)
+            if guided:                                                            # the round's pair is e_next in round 1, e_t after it
+                new = 1 if j == 1 else 0
+                hist, cf = eps_list[:new] + eps_list[new + 1:], [coefs[new]] + coefs[:new] + coefs[new + 1:]
+                cur, e_new = update_guided(cur, eps_list[new], hist, cf, draw(cur, b), j, b, 1 < j < R - 1)
+                if j > 1:
+                    e_t = e_new
+            else:
+                cur = update(cur, eps_list, coefs, draw(cur, b), j, b)
             old_eps.append(e_t)
             if len(old_eps) >= 4:
                 old_eps.pop(0)
