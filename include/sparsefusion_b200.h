@@ -238,7 +238,8 @@ int sfb_gate_residual_nhwc(const float* h, int64_t ldh, const float* gate, const
 
 /* PLMSSampler.p_sample tail (external/plms.py:143-154, :183-212) as one elementwise pass over the latent:
  *   e' = c0*e0 + c1*e1 + c2*e2 + c3*e3 (e1..e3 may be NULL);  x0 = clamp((x - sigma*e') / max(alpha,1e-8), +-clip);
- *   x_prev = alpha_next * (x*(1-c)/alpha + c*x0) + noise_scale * noise.   x0_out / e_out may be NULL. */
+ *   x_prev = alpha_next * (x*(1-c)/alpha + c*x0) + noise_scale * noise.   x0_out / e_out may be NULL.
+ * The clamp keeps NaN, as torch.clamp does: a NaN eps or x gives a NaN x0 and x_prev, never a value at +-clip. */
 int sfb_plms_update(const float* x, const float* e0, const float* e1, const float* e2, const float* e3, float c0, float c1, float c2,
                     float c3, const float* noise, float alpha, float sigma, float alpha_next, float c, float noise_scale, float clip,
                     float* x_prev, float* x0_out, float* e_out, int64_t n, void* stream);
@@ -261,6 +262,7 @@ int sfb_plms_update_rows_cfg(const float* x, const float* e_cond, const float* e
  *   e = cond_scale*e_cond + (1-cond_scale)*e_null (e_null may be NULL: e = e_cond);  x0 = (x - sigma*e) / max(alpha,1e-8);
  *   s = max(torch.quantile(|x0|, percentile, 'linear'), 1) per row, computed exactly;  x0 = clamp(x0, +-s) / s;
  *   x_prev = alpha_next * (x*(1-c)/alpha + c*x0) + noise_scale * noise.
+ * NaN follows torch: a row whose x0 holds a NaN has s = NaN and an all-NaN x_prev.
  * s_out [B] receives s, x0_out the unthresholded x0; either may be NULL.  x_prev must not alias the inputs. */
 int sfb_ddpm_dynamic_step(const float* x, const float* e_cond, const float* e_null, float cond_scale, const float* noise, float alpha,
                           float sigma, float alpha_next, float c, float noise_scale, float percentile, int row_len, int B, float* x_prev,
@@ -395,7 +397,7 @@ int sfb_lpips_head(const float* f0, const float* f1, const float* w, int HW, int
  *    utils/eft_renderer.py.  ResNet-18 convolutions (BatchNorm folded) and every nn.Linear of the three transformer encoders use
  *    sfb_conv2d_nhwc_tf32_ex; these are the NHWC fp32 operators around them.  sparsefusion_b200/eft.py strings them together.
  * ========================================================================================== */
-/* torchvision resnet maxpool: 3x3 window, stride 2, padding 1; y [NB][(H+1)/2][(W+1)/2][C] */
+/* torchvision resnet maxpool: 3x3 window, stride 2, padding 1; y [NB][(H+1)/2][(W+1)/2][C]; a NaN in a window gives NaN (F.max_pool2d) */
 int sfb_maxpool3x3s2_nhwc(const float* x, float* y, int NB, int H, int W, int C, void* stream);
 /* F.interpolate(mode='bilinear', align_corners=True) to (Ho, Wo), written with channel stride ldo (eft.py:194-202 pyramid concatenation) */
 int sfb_resize_bilinear_ac_nhwc(const float* x, int64_t ldx, float* y, int64_t ldo, int NB, int H, int W, int C, int Ho, int Wo, void* stream);
@@ -405,7 +407,7 @@ int sfb_grid_sample_nhwc(const float* x, int64_t ldx, const float* grid, float* 
 /* single-head attention core of nn.TransformerEncoderLayer(d_model E, nhead 1), sequence-first: qkv [S][B][3E] = in_proj(x) (q | k | v),
  * out [S][B][E] = softmax(q k^T / sqrt(E)) v over the S <= 32 positions of each batch element (eft.py:30-33: S = input views or depth samples) */
 int sfb_seq_attention(const float* qkv, float* out, int S, int B, int E, void* stream);
-/* in place over n floats (n % 4 == 0): kind 0 ReLU, 1 GELU (erf) */
+/* in place over n floats (n % 4 == 0): kind 0 ReLU (NaN stays NaN, as F.relu), 1 GELU (erf) */
 int sfb_act_inplace(float* x, int64_t n, int kind, void* stream);
 /* the T1 token rows of the view-batched feature cache (eft.py:215-327, what EpipolarFeatureTransformer.forward assembles in eager passes), for
  * V query views with their own NC input cameras each: cams [V][NC][16] = R row-major (9) | T (3) | focal (2) | principal point (2) in pytorch3d's

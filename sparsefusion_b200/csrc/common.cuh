@@ -72,6 +72,11 @@ static inline void trace_bind_this_tu(unsigned long long* buf, unsigned int cap)
 }
 __device__ __forceinline__ void pdl_sync() { pdl_trigger(); pdl_wait(); trace_mark(); }
 
+// torch.clamp, max pooling and relu keep a NaN operand; fminf / fmaxf return the other operand instead.  On operands that are not NaN
+// these are fminf / fmaxf, bit for bit (signed zeros included).
+__device__ __forceinline__ float clamp_keep_nan(float x, float lo, float hi) { return x != x ? x : fminf(fmaxf(x, lo), hi); }
+__device__ __forceinline__ float max_keep_nan(float a, float b) { return (a != a || b != b) ? a + b : fmaxf(a, b); }
+
 // cluster_x > 1 launches thread-block clusters of (cluster_x, 1, 1); grid.x must be a multiple of it
 template <typename... KA, typename... A>
 static inline cudaError_t launch_pdl_cluster(void (*kernel)(KA...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, unsigned cluster_x,

@@ -10,7 +10,8 @@
 
 namespace sfb {
 
-// y[n][oh][ow][c] = max over the 3x3 window at stride 2, padding 1 (torchvision resnet maxpool; padded positions never win)
+// y[n][oh][ow][c] = max over the 3x3 window at stride 2, padding 1 (torchvision resnet maxpool; padded positions never win; a NaN in the
+// window gives NaN, as F.max_pool2d does)
 __global__ void maxpool3x3s2_kernel(const float4* __restrict__ x, float4* __restrict__ y, int H, int W, int Ho, int Wo, int C4, int64_t total) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
         const int c = (int)(i % C4);
@@ -28,7 +29,7 @@ __global__ void maxpool3x3s2_kernel(const float4* __restrict__ x, float4* __rest
                 const int iw = ow * 2 - 1 + dx;
                 if (iw < 0 || iw >= W) continue;
                 const float4 v = __ldg(x + (((int64_t)n * H + ih) * W + iw) * C4 + c);
-                m.x = fmaxf(m.x, v.x); m.y = fmaxf(m.y, v.y); m.z = fmaxf(m.z, v.z); m.w = fmaxf(m.w, v.w);
+                m.x = max_keep_nan(m.x, v.x); m.y = max_keep_nan(m.y, v.y); m.z = max_keep_nan(m.z, v.z); m.w = max_keep_nan(m.w, v.w);
             }
         }
         y[i] = m;
@@ -215,12 +216,12 @@ __global__ void __launch_bounds__(256) seq_attention_kernel(const float* __restr
     }
 }
 
-// in place: kind 0 = ReLU, 1 = GELU (erf form, nn.GELU default)
+// in place: kind 0 = ReLU (NaN stays NaN, as F.relu), 1 = GELU (erf form, nn.GELU default)
 __global__ void act_inplace_kernel(float4* __restrict__ x, int64_t n4, int kind) {
     for (int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x; i < n4; i += (int64_t)gridDim.x * blockDim.x) {
         float4 v = x[i];
         if (kind == 0) {
-            v.x = fmaxf(v.x, 0.f); v.y = fmaxf(v.y, 0.f); v.z = fmaxf(v.z, 0.f); v.w = fmaxf(v.w, 0.f);
+            v.x = max_keep_nan(v.x, 0.f); v.y = max_keep_nan(v.y, 0.f); v.z = max_keep_nan(v.z, 0.f); v.w = max_keep_nan(v.w, 0.f);
         } else {
             v.x = 0.5f * v.x * (1.f + erff(v.x * 0.70710678118654752f)); v.y = 0.5f * v.y * (1.f + erff(v.y * 0.70710678118654752f));
             v.z = 0.5f * v.z * (1.f + erff(v.z * 0.70710678118654752f)); v.w = 0.5f * v.w * (1.f + erff(v.w * 0.70710678118654752f));

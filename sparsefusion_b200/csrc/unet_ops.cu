@@ -1366,7 +1366,7 @@ __device__ __forceinline__ void plms_update_value(int64_t i, float e0v, const fl
     if (e3) e += c3 * e3[i];
     const float xv = x[i];
     float x0 = (xv - sigma * e) / fmaxf(alpha, 1e-8f);
-    x0 = fminf(fmaxf(x0, -clip), clip);
+    x0 = clamp_keep_nan(x0, -clip, clip);     // a NaN eps or x gives a NaN x0 and x_prev, as torch.clamp does
     const float mean = alpha_next * (xv * (1.f - c) / alpha + c * x0);
     x_prev[i] = mean + noise_scale * noise[i];
     if (x0_out) x0_out[i] = x0;
@@ -1484,7 +1484,8 @@ extern "C" int sfb_plms_update_rows_cfg(const float* x, const float* e_cond, con
 // The quantile is exact: |x0| >= 0, so the order of its uint32 bit patterns is the order of the values, and a 4-pass radix select on 8-bit digits
 // finds the value of rank floor(p * (n - 1)) without sorting; the next rank is either the same value (ties) or the least value above it.  A row
 // is split over a thread-block cluster of up to 8 CTAs (kDynChunk floats each, held in shared memory); their digit histograms are summed
-// through distributed shared memory, as in gn_cluster_kernel.
+// through distributed shared memory, as in gn_cluster_kernel.  NaN patterns sort above +inf; torch.quantile returns NaN for a row that holds
+// a NaN, so pass 0's histogram has a 257th bin counting them, and such a row gets s = NaN (and an all-NaN x_prev, as clamp / s gives).
 namespace sfb {
 constexpr int kDynThreads = 1024;
 constexpr int kDynChunk = 8192;       // floats of a row per CTA: 32 KB of shared memory
@@ -1503,8 +1504,8 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
     float* __restrict__ x_prev, float* __restrict__ s_out, float* __restrict__ x0_out) {
     pdl_sync();
     extern __shared__ float x0s[];                 // this CTA's slice of the row's x0
-    __shared__ unsigned hist[2][256];              // digit histogram, double-buffered so that one cluster barrier per pass suffices
-    __shared__ unsigned tot[256];
+    __shared__ unsigned hist[2][257];              // digit histogram (+ NaN count), double-buffered so that one cluster barrier per pass suffices
+    __shared__ unsigned tot[257];
     __shared__ unsigned sel[3];                    // selected digit, rank left within it, its count
     __shared__ unsigned vmin;
     unsigned k = 1, crank = 0;
@@ -1517,7 +1518,7 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
     const int i0 = min(row_len, (int)crank * chunk), len = min(row_len, i0 + chunk) - i0;
     const int64_t base = (int64_t)blockIdx.y * row_len + i0;
     const int lane = threadIdx.x & 31;
-    for (int i = threadIdx.x; i < 512; i += blockDim.x) (&hist[0][0])[i] = 0u;
+    for (int i = threadIdx.x; i < 2 * 257; i += blockDim.x) (&hist[0][0])[i] = 0u;
     if (threadIdx.x == 0) vmin = 0xffffffffu;
 
     const float cn = 1.f - cond_scale;
@@ -1535,6 +1536,7 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
     const int klo = (int)rk, khi = (int)ceilf(rk);
     const float w = rk - (float)klo;
     unsigned prefix = 0u, want = (unsigned)klo, cnt_eq = 0u;
+    bool has_nan = false;
     const int iters = (len + blockDim.x - 1) / blockDim.x;
 #pragma unroll 1
     for (int pass = 0; pass < 4; ++pass) {
@@ -1549,9 +1551,13 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
             const unsigned d = (u >> shift) & 255u;
             const unsigned peers = __match_any_sync(0xffffffffu, m ? d : 0xffffffffu);   // lanes with the same digit add once
             if (m && lane == __ffs(peers) - 1) atomicAdd(&h[d], (unsigned)__popc(peers));
+            if (pass == 0) {
+                const unsigned nans = __ballot_sync(0xffffffffu, i < len && u > 0x7f800000u);
+                if (nans && lane == 0) atomicAdd(&h[256], (unsigned)__popc(nans));
+            }
         }
         dyn_sync<CLUSTER>();                                       // every CTA's histogram of this pass is complete
-        for (int b = threadIdx.x; b < 256; b += blockDim.x) {
+        for (int b = threadIdx.x; b < 257; b += blockDim.x) {
             unsigned s = 0u;
             if (CLUSTER) {
                 cg::cluster_group cl = cg::this_cluster();
@@ -1562,7 +1568,7 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
             tot[b] = s;
         }
         // every peer finished reading the other buffer before it reached the barrier above: clear it for the next pass
-        for (int b = threadIdx.x; b < 256; b += blockDim.x) hist[(pass + 1) & 1][b] = 0u;
+        for (int b = threadIdx.x; b < 257; b += blockDim.x) hist[(pass + 1) & 1][b] = 0u;
         __syncthreads();
         if (threadIdx.x < 32) {                                    // find the digit holding rank `want`: 8 bins per lane, warp prefix sum
             unsigned v[8], sum = 0u;
@@ -1584,6 +1590,7 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
             }
         }
         __syncthreads();
+        if (pass == 0) has_nan = tot[256] != 0u;
         prefix |= sel[0] << shift;
         want = sel[1];
         cnt_eq = sel[2];
@@ -1610,11 +1617,11 @@ __global__ void __launch_bounds__(kDynThreads) ddpm_dynamic_step_kernel(
     if (CLUSTER) asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");   // done reading the peers' shared memory ...
     const float dv = vhi - vlo;
     // lerp(vlo, vhi, w) exactly as ATen/native/Lerp.h compiles for CUDA (the product and the add contract to one fma)
-    const float q = fabsf(w) < 0.5f ? __fmaf_rn(w, dv, vlo) : __fmaf_rn(-dv, 1.f - w, vhi);
-    const float s = fmaxf(q, 1.f);
+    const float q = has_nan ? __uint_as_float(0x7fffffffu) : (fabsf(w) < 0.5f ? __fmaf_rn(w, dv, vlo) : __fmaf_rn(-dv, 1.f - w, vhi));
+    const float s = q != q ? q : fmaxf(q, 1.f);                    // .clamp(min=1) keeps NaN
     if (s_out && crank == 0 && threadIdx.x == 0) s_out[blockIdx.y] = s;
     for (int i = threadIdx.x; i < len; i += blockDim.x) {
-        const float x0 = fminf(fmaxf(x0s[i], -s), s) / s;
+        const float x0 = clamp_keep_nan(x0s[i], -s, s) / s;
         const float xv = x[base + i];
         const float mean = alpha_next * (xv * (1.f - c) / alpha + c * x0);
         x_prev[base + i] = mean + noise_scale * noise[base + i];

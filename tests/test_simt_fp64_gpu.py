@@ -12,8 +12,8 @@ tensor and the channels between a slice and its row stride), the GroupNorm works
 stay bit-identical.  The tracer names the kernels that ran; they must equal ``kernel_plan``.  Kernels with a fixed fold order run twice and
 must agree bit for bit.
 
-Out of scope: GEMMs (tests/test_conv_fp64_gpu.py), plms_update / ddpm_dynamic_step, image_glue.cu, the EFT-only kernels of eft_ops.cu and
-ordering hazards between launches."""
+Out of scope: GEMMs (tests/test_conv_fp64_gpu.py), the sampler updates, image_glue.cu and the EFT-only kernels of eft_ops.cu
+(tests/test_step_fp64_gpu.py) and ordering hazards between launches."""
 import ctypes
 import math
 from collections import defaultdict
