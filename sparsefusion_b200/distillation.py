@@ -32,6 +32,7 @@ permutation, all-reduce, Adam with grad_scale 1/R) that ``tests/test_multirank_g
 """
 from __future__ import annotations
 
+import math
 from dataclasses import dataclass
 from typing import Optional
 
@@ -40,7 +41,15 @@ import torch.nn.functional as F
 
 from . import _lib as lib
 from . import image_glue as glue
-from .plms import PLMSSampler, _log_snr as plms_log_snr, _sigmoid as plms_sigmoid
+from .plms import PLMSSampler, _log_snr as plms_log_snr, _sigmoid as plms_sigmoid, check_cond_scale
+
+
+def _check_cond_scale(vldm, cond_scale, where):
+    """ValueError, before any device work, for a guidance scale of the SDS target that is not finite, or not 1 on a VLDM without
+    conditional dropout"""
+    if not math.isfinite(float(cond_scale)):
+        raise ValueError(f'{where}: cond_scale must be finite (got {cond_scale!r})')
+    check_cond_scale(vldm, cond_scale, where)
 
 
 def normalize(x):  # utils/common_utils.py:9-13
@@ -191,7 +200,9 @@ class FlatAdam:
 class Distiller:
     def __init__(self, ngp, vae, vldm, opt, cache: SceneCache, *, z_scale_factor=0.18215, plms_steps=50, start_fusion_step=1000,
                  lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3, seed=0, rank=0, world_size=1, process_group=None,
-                 use_cuda_graph=True, fused_glue=True, percep=None, lambda_percep=0.1, start_percep_step=1000, views_per_step=None, max_batch=32):
+                 use_cuda_graph=True, fused_glue=True, percep=None, lambda_percep=0.1, start_percep_step=1000, views_per_step=None, max_batch=32,
+                 cond_scale=1.0):
+        _check_cond_scale(vldm, cond_scale, 'Distiller')
         self.ngp, self.vae, self.vldm, self.opt, self.cache = ngp, vae, vldm, opt, cache
         self.z_scale_factor = z_scale_factor
         self.start_fusion_step = start_fusion_step
@@ -200,6 +211,8 @@ class Distiller:
         # None: the reference's two-update iteration on one view (one rank) / one view per rank (N ranks, legacy form); V: view-batched minibatch step
         self.views_per_step = views_per_step
         self.max_batch = max_batch     # views per VAE / PLMS batch on one rank (activations of the VAE decoder: 0.27 GB per tensor per 8 views at 256^2)
+        # classifier-free guidance scale of the SDS target's PLMS run (1: none); with guidance the UNet evaluates 2 rows per view
+        self.cond_scale = float(cond_scale)
         self.seed = seed
         # perceptual term (distillation.py:161, :176-178, :312-314): a PerceptualLoss module (lpips_vgg.py) or None; lambda switches on at start_percep_step
         self.percep, self.lambda_percep, self.start_percep_step = percep, lambda_percep, start_percep_step
@@ -358,18 +371,20 @@ class Distiller:
     def _fusion_target(self, images, feats, max_thres, noise_fn, sampler=None):
         """the denoised targets of a batch of renders ([C>=3,H,W] each, colour first): VAE encode (:299), PLMS sampling (:304), decode (:309).
         Returns (pred_img [B,3,H,W], alpha_cumprod [B] of the run's first noise level, fp32).  ``max_thres`` is one float shared by the batch
-        (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows``); ``noise_fn`` serves the run's draws, None: the sampler's own."""
+        (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows``); ``noise_fn`` serves the run's draws, None: the sampler's own.
+        The run is guided with ``self.cond_scale``."""
         sampler = self.sampler if sampler is None else sampler
         batch = images[0][None, :3] if len(images) == 1 else torch.stack([im[:3] for im in images])
         latents = self.vae.encode(normalize(batch)).mode() * self.z_scale_factor                # :299
         if isinstance(max_thres, (list, tuple)):
-            out = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn)
+            out = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn, cond_scale=self.cond_scale)
         else:
             prev = sampler.noise_fn
             if noise_fn is not None:
                 sampler.noise_fn = noise_fn
             try:
-                out = sampler.sample(latents, cond_images=feats, use_tqdm=False, return_noise=True, max_thres=max_thres)   # :304
+                out = sampler.sample(latents, cond_images=feats, cond_scale=self.cond_scale, use_tqdm=False, return_noise=True,
+                                     max_thres=max_thres)                                                             # :304
             finally:
                 sampler.noise_fn = prev
         return unnormalize(self.vae.decode(1.0 / self.z_scale_factor * out[0])).clip(0.0, 1.0), out[3]     # :309
@@ -457,6 +472,11 @@ class MultiSceneDistiller:
     (each scene at its own noise level, so with its own number of UNet evaluations; the UNet runs at the batch of scenes still sampling) and
     ONE decode, in chunks of at most ``max_batch`` scenes.  The SDS phase's UNet and VAE run at batch S instead of S times at batch 1.
 
+    ``cond_scale`` guides every scene's SDS target with the same classifier-free guidance scale (1: none; ValueError at construction when the
+    VLDM has no conditional dropout).  ``max_batch`` counts scenes, guided or not: a guided chunk of b scenes still sampling evaluates its
+    conditional and null rows as one UNet batch of 2b rows, so the sampler's CUDA graphs cover the batch sizes 1..max_batch unguided and
+    2, 4, .., 2 * max_batch guided, each captured when a run first reaches it.
+
     Draws of scene k: the view permutation and ``u`` from ``torch.Generator().manual_seed(seeds[k])`` in the reference's order (as in
     ``Distiller(seed=seeds[k])``); the render jitter / inverse-CDF samples of the photometric render from ``view_seed(seeds[k], itr, 0, 0)``, those
     of the fusion render of view v from ``view_seed(seeds[k], itr, v, 1)`` and the PLMS noise from ``view_seed(seeds[k], itr, v, 2)``.  A scene's
@@ -466,7 +486,8 @@ class MultiSceneDistiller:
     Not supported: ``views_per_step`` (NotImplementedError), ``fused_glue=False`` and ``opt.hw_scale != 2`` (NotImplementedError), scenes of
     different image, latent or ray sizes (ValueError), CPU tensors (RuntimeError)."""
 
-    def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, **kw):
+    def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, cond_scale=1.0, **kw):
+        _check_cond_scale(vldm, cond_scale, 'MultiSceneDistiller')
         if kw.get('views_per_step') is not None:
             raise NotImplementedError('MultiSceneDistiller runs the reference iteration (one target view per scene); views_per_step is not supported')
         if not kw.get('fused_glue', True) or int(opt.hw_scale) != 2:
@@ -484,14 +505,16 @@ class MultiSceneDistiller:
                 if tuple(t.shape[1:]) != tuple(getattr(caches[0], f).shape[1:]):
                     raise ValueError(f'MultiSceneDistiller: scenes differ in SceneCache.{f} size ({tuple(t.shape[1:])} vs '
                                      f'{tuple(getattr(caches[0], f).shape[1:])}); batched scenes need equal image, latent and ray sizes')
-        self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, **kw) for ngp, cache, sd in zip(ngps, caches, seeds)]
+        self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, cond_scale=cond_scale, **kw)
+                       for ngp, cache, sd in zip(ngps, caches, seeds)]
         for d in self.scenes:
             d._keyed = True
         self.seeds = [int(s) for s in seeds]
         self.max_batch = int(max_batch)
+        self.cond_scale = float(cond_scale)
         lead = self.scenes[0]
         self.start_fusion_step = lead.start_fusion_step
-        # one sampler for all scenes: its UnetGraph holds one graph per batch size (at most max_batch of them)
+        # one sampler for all scenes: its UnetGraph holds one graph per UNet batch size (at most max_batch of them: see the class docstring)
         self.sampler = PLMSSampler(vldm, lead.sampler.plms_steps, use_cuda_graph=lead.sampler.use_cuda_graph)
         self.render_noise = None
         self.plms_noise = None     # parity tests: callable(scene) -> noise_fn(like) serving that scene's PLMS draws
@@ -739,7 +762,8 @@ class NativeSceneBuilder:
 
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
-                      process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0):
+                      process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
+                      cond_scale=1.0):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -772,8 +796,15 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     the scene views after the loop (``baselines.evaluate_baselines``): the cached EFT images and VLDM samples from pure noise conditioned on
     the cached EFT features (guidance scale ``vldm_cond_scale``, draws keyed by the scene's seed), with the same metrics as ``evaluate``, and
     writes ``{save_dir}/metrics/{seq_name}_eft.txt``, ``{seq_name}_vldm.txt`` and ``{save_dir}/render_gifs/{seq_name}_baselines.gif``.
+
+    ``cond_scale`` is the classifier-free guidance scale of the distillation itself: every SDS target is sampled with
+    eps = null + (cond - null) * cond_scale, the conditional and null branches as one UNet batch (1, the default, is the reference's unguided
+    loop).  It is independent of ``vldm_cond_scale``, which only guides the VLDM baseline's samples.  Guidance needs a VLDM trained with
+    conditional dropout (ValueError before any work otherwise); with ``use_diffusion=False`` there is no SDS target and it is ignored.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
+    if use_diffusion:
+        _check_cond_scale(vldm, cond_scale, 'distillation_loop')
     rank, world = 0, 1
     if process_group is not None:
         rank, world = torch.distributed.get_rank(process_group), torch.distributed.get_world_size(process_group)
@@ -781,7 +812,7 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     def make(ngps, caches, percep, seed):
         return Distiller(ngps[0], vae, vldm, opt, caches[0], plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0,   # :148-160
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
-                         start_percep_step=1000, views_per_step=views_per_step)
+                         start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
                                      visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
@@ -790,7 +821,8 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
-                   evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0):
+                   evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
+                   cond_scale=1.0):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -801,14 +833,17 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     ``{save_dir}/metrics/{seq_name}.txt`` written as ``distillation_loop(evaluate=True)`` does, scene k's render jitter keyed by ``seed + k``.
     ``visualize`` / ``visualize_shadings``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter
     keyed by ``seed + k``.  ``evaluate_baselines`` / ``vldm_cond_scale``: each scene's EFT and VLDM baselines scored and written as
-    ``distillation_loop(evaluate_baselines=True)`` does, scene k's VLDM draws keyed by ``seed + k``.
+    ``distillation_loop(evaluate_baselines=True)`` does, scene k's VLDM draws keyed by ``seed + k``.  ``cond_scale``: the guidance scale of
+    every scene's SDS targets, as ``distillation_loop(cond_scale=...)``, independent of ``vldm_cond_scale``.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
+    if use_diffusion:
+        _check_cond_scale(vldm, cond_scale, 'distill_scenes')
 
     def make(ngps, caches, percep, base):
         return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
-                                   lambda_percep=0.1, start_percep_step=1000)
+                                   lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
                              loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
 

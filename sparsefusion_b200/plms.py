@@ -17,8 +17,8 @@ each evaluation is ONE batch-2B graph replay of the conditional and null rows, a
 (``sfb_plms_update_rows_cfg``), as ``DDPM.sample`` does it.
 
 ``sample_rows`` runs a batch whose rows each have their own ``max_thres`` (scene-batched distillation): the rows share every round of UNet
-evaluation while they are still running (``RowSchedule``), and the update kernel takes its scalars per row (``sfb_plms_update_rows``).  The same
-loop serves ``sample``, where every row shares one schedule.
+evaluation while they are still running (``RowSchedule``), and the update kernel takes its scalars per row (``sfb_plms_update_rows``, or
+``sfb_plms_update_rows_cfg`` with guidance).  The same loop serves ``sample``, where every row shares one schedule.
 """
 from __future__ import annotations
 
@@ -75,7 +75,8 @@ def _row_lin(max_thres: float, plms_steps: int) -> list:
 class RowSchedule:
     """the batched run of S rows that each follow their own PLMS schedule.
 
-    Round j is one UNet evaluation followed by one ``sfb_plms_update_rows`` launch.  A row of n >= 1 steps takes part in rounds 0..n: round 0
+    Round j is one UNet evaluation followed by one ``sfb_plms_update_rows`` launch (guided: one evaluation of the active rows' conditional and
+    null pairs, followed by one ``sfb_plms_update_rows_cfg`` launch).  A row of n >= 1 steps takes part in rounds 0..n: round 0
     evaluates e_t at lin[0] and makes the pseudo improved Euler predictor x_prev, round 1 evaluates e_next at lin[1] and completes step 0, round
     j >= 2 is step j - 1 (Adams-Bashforth).  So a row makes n + 1 evaluations, as the single-row sampler does, and a row of n = 0 none.  Rows are
     sorted by descending n (stable), which makes the active rows of every round a prefix ``[0, batch[j])`` of the sorted order."""
@@ -123,6 +124,14 @@ def row_schedule(max_thres: Sequence[float], plms_steps: int) -> RowSchedule:
         scalars.append(sc)
     calls = [n + 1 if n > 0 else 0 for n in ns]
     return RowSchedule(order, ns, lins, batch, levels, level_idx, scalars, calls)
+
+
+def check_cond_scale(diffusion, cond_scale, where: str):
+    """ValueError, before any device work, for classifier-free guidance (``cond_scale != 1``) on a VLDM built without conditional dropout
+    (``cond_drop_prob == 0``): its null branch was never trained"""
+    if cond_scale != 1 and not diffusion.can_classifier_guidance:
+        raise ValueError(f'{where}: the VLDM was not trained with conditional dropout (cond_drop_prob == 0), so classifier-free '
+                         f'guidance (cond_scale {cond_scale} != 1) is not available')
 
 
 class PLMSSampler:
@@ -175,9 +184,7 @@ class PLMSSampler:
         branches are one batch-2B UNet evaluation (``_eps_pair``) and the guided eps is formed inside the step's update kernel.  Refused
         (ValueError) when the VLDM was built without conditional dropout (``cond_drop_prob == 0``), as ``DDPM.sample`` refuses it."""
         d = self.diffusion
-        if cond_scale != 1 and not d.can_classifier_guidance:
-            raise ValueError('PLMSSampler.sample: the VLDM was not trained with conditional dropout (cond_drop_prob == 0), so classifier-free '
-                             f'guidance (cond_scale {cond_scale} != 1) is not available')
+        check_cond_scale(d, cond_scale, 'PLMSSampler.sample')
         batch_size = cond_images.shape[0]
         shape = (batch_size, d.sample_channels[0], d.image_sizes[0], d.image_sizes[0])
         img, x_noisy, noise, alpha_cumprod = self.plms_sample_loop(d.unets[0], image=image, shape=shape, cond_images=cond_images,
@@ -225,16 +232,21 @@ class PLMSSampler:
         return self.diffusion.unnormalize_img(img), x_noisy, noise, torch.sigmoid(log_snr)
 
     @torch.no_grad()
-    def sample_rows(self, image, max_thres: Sequence[float], cond_images, noise_fn=None):
+    def sample_rows(self, image, max_thres: Sequence[float], cond_images, noise_fn=None, cond_scale=1.0):
         """one batched run in which row k follows the schedule of its own ``max_thres[k]``: the same result per row as ``sample(image[k:k+1],
-        max_thres[k], cond_images[k:k+1], return_noise=True)``, with rows that are still running sharing each UNet evaluation.  Returns
-        ``(pred_x0, x_noisy, noise, alpha_cumprod)`` in the caller's row order.
+        max_thres[k], cond_images[k:k+1], cond_scale=cond_scale, return_noise=True)``, with rows that are still running sharing each UNet
+        evaluation.  Returns ``(pred_x0, x_noisy, noise, alpha_cumprod)`` in the caller's row order.
+
+        ``cond_scale != 1``: classifier-free guidance with one scale for every row.  A round evaluates the latents of its b active rows twice,
+        with their conditioning and with zeros, as ONE batch-2b UNet evaluation; ValueError when the VLDM has no conditional dropout.
 
         ``noise_fn(like, rows=None)`` serves every Gaussian draw: row i of the result belongs to caller row ``rows[i]`` (all rows, in order, when
-        ``rows`` is None).  Each row draws in the single-row sampler's order and count; a finished row draws nothing.  Defaults to
-        ``self.noise_fn``, which may ignore ``rows`` when the draws need not be reproducible per row.  ``last_unet_calls`` counts the batched
-        evaluations, ``last_row_calls`` the evaluations of each row, ``last_graph_replays`` the evaluations replayed from a CUDA graph."""
+        ``rows`` is None).  Each row draws in the single-row sampler's order and count, guided or not; a finished row draws nothing.  Defaults
+        to ``self.noise_fn``, which may ignore ``rows`` when the draws need not be reproducible per row.  ``last_unet_calls`` counts the batched
+        evaluations, ``last_row_calls`` the evaluations of each row (a guided row's conditional and null pair counts once),
+        ``last_graph_replays`` the evaluations replayed from a CUDA graph."""
         d = self.diffusion
+        check_cond_scale(d, cond_scale, 'PLMSSampler.sample_rows')
         if not image.is_cuda:
             raise RuntimeError('PLMSSampler.sample_rows runs on CUDA tensors only')
         if d.pred_objectives[0] != 'noise' or d.dynamic_thresholding[0] or not d.clip_output:
@@ -248,7 +260,7 @@ class PLMSSampler:
         if noise_fn is not None:
             self.noise_fn = noise_fn
         try:
-            return self._fused_loop(d.unets[0], image.float().contiguous(), cond_images, 1.0, [float(m) for m in max_thres])
+            return self._fused_loop(d.unets[0], image.float().contiguous(), cond_images, cond_scale, [float(m) for m in max_thres])
         finally:
             self.noise_fn = prev
 
@@ -256,16 +268,14 @@ class PLMSSampler:
     def _fused_loop(self, unet, image, cond_images, cond_scale, max_thres):
         """plms_sample_loop (:54-119) + p_sample (:122-156) with the per-step latent math in one kernel.  ``max_thres`` is one float (every row
         runs the same schedule: ``sample``) or one float per row (``sample_rows``); see ``RowSchedule`` for how rows of different lengths share
-        the rounds.  Guided (``cond_scale != 1``, one schedule only): each round evaluates the rows cat(x, x) with cat(cond, cond * 0) as one
-        UNet batch and ``sfb_plms_update_rows_cfg`` forms the guided eps in front of the Adams-Bashforth combination; the history keeps the
-        guided eps the kernel writes out, as the reference's p_sample returns it."""
+        the rounds.  Guided (``cond_scale != 1``): each round evaluates its b active rows cat(x, x) with cat(cond, cond * 0) as one UNet batch
+        of 2b rows and ``sfb_plms_update_rows_cfg`` forms the guided eps of each row, with that row's scalars, in front of the Adams-Bashforth
+        combination; the history keeps the guided eps the kernel writes out, as the reference's p_sample returns it."""
         S = image.shape[0]
         dev = image.device
         clip = float(self.diffusion.clip_value)
         same = not isinstance(max_thres, (list, tuple))
         guided = cond_scale != 1
-        if guided and not same:
-            raise NotImplementedError('PLMSSampler: classifier-free guidance runs with one schedule for every row (sample), not per-row schedules')
         mts = [float(max_thres)] * S if same else list(max_thres)
         same = same or len(set(mts)) == 1
         sch = row_schedule(mts, self.plms_steps)
@@ -293,10 +303,13 @@ class PLMSSampler:
         levels_ls = take(len(sch.levels))
         a0_t, s0_t, acp_t, hi_t = (take(S).view(S, 1, 1, 1) for _ in range(4))
         if not identity or not all(len(set(idx)) == 1 for idx in sch.level_idx):
-            ibuf = torch.tensor(order + [0] * S + [i for idx in sch.level_idx for i in idx + [0] * (S - len(idx))], dtype=torch.int64)
+            # level of each evaluated row per round: guided rounds evaluate the active rows twice (conditional, then null)
+            lvl_rows = [idx + idx if guided else idx for idx in sch.level_idx]
+            W = 2 * S if guided else S
+            ibuf = torch.tensor(order + [0] * S + [i for idx in lvl_rows for i in idx + [0] * (W - len(idx))], dtype=torch.int64)
             ibuf[S + torch.tensor(order)] = torch.arange(S)                      # inverse permutation
             ibuf = ibuf.pin_memory().to(dev, non_blocking=True)
-            perm_d, inv_d, lvl_tab = ibuf[:S], ibuf[S:2 * S], ibuf[2 * S:].view(R, S)
+            perm_d, inv_d, lvl_tab = ibuf[:S], ibuf[S:2 * S], ibuf[2 * S:].view(R, W)
 
         noise = self.noise_fn(image)                                              # plms.py:89/91: every row draws its q_sample noise
         if same:                                                                  # one schedule: scalar arithmetic, exactly as the single-row run
@@ -308,9 +321,14 @@ class PLMSSampler:
             img = torch.where(hi_t > 0.5, image, x_noisy)
         cur = img if identity else img.index_select(0, perm_d)
         cond = cond_images if identity else cond_images.index_select(0, perm_d)
-        if guided:                                                                # the conditional rows, then the null rows (every round has S rows)
-            cond = torch.cat((cond, torch.zeros_like(cond))).contiguous()
+        cond_pairs = {}                                                           # guided: batch b -> the conditional rows [:b], then b null rows
         row_len = image[0].numel()
+
+        def cond_pair(b):
+            # fixed per batch size for the whole run, as the graph's conditioning share requires (_replay)
+            if b not in cond_pairs:
+                cond_pairs[b] = torch.cat((cond[:b], torch.zeros_like(cond[:b]))).contiguous()
+            return cond_pairs[b]
 
         # the run's noise levels are known now: everything of the UNet that depends on them only (time embedding, conditioning tokens, all
         # time MLPs) is evaluated for the whole run in one batch (Unet.precompute_time) instead of once per evaluation
@@ -332,9 +350,9 @@ class PLMSSampler:
                 if len(set(idx)) == 1:
                     tf = {k: v[idx[0]:idx[0] + 1].expand(nb, *v.shape[1:]) for k, v in tf_all.items()}
                 else:
-                    tf = {k: v.index_select(0, lvl_tab[j, :b]) for k, v in tf_all.items()}
+                    tf = {k: v.index_select(0, lvl_tab[j, :nb]) for k, v in tf_all.items()}
             if guided:
-                return self._eps_pair(unet, torch.cat((x, x)), ls_tab[j, :b].repeat(2) if tf is None else None, cond, tf)
+                return self._eps_pair(unet, torch.cat((x, x)), ls_tab[j, :b].repeat(2) if tf is None else None, cond_pair(b), tf)
             return self._eps(unet, x, ls_tab[j, :b], cond[:b], cond_scale, time_features=tf)
 
         def update_guided(x, pair, hist, coefs, z, j, b, keep):
