@@ -314,26 +314,46 @@ int sfb_ngp_field_normal_backward(const float* xyz, const float* rays_o, const f
                                   const float* b0, const float* W1, const float* b1, const float* W2, const float* b2, float eps,
                                   const float* fd, const float* grad_normal, const float* grad_fd, float* grad_embeddings, float* gW0,
                                   float* gb0, float* gW1, float* gb1, float* gW2, float* gb2, void* stream);
-/* The per-ray stages of NeRFRenderer.run (external/nerf/renderer_df.py:310-468; num_steps = upsample_steps = 64), one warp per ray.
- * All random draws of the reference are inputs: noise [N,64] U(0,1) or NULL (perturb=False, :363); u [N,64] (torch.rand at :31, or the
- * deterministic linspace of :28 in eval mode).  lin = torch.linspace(0,1,64) (:356), passed in so depths are bit-identical to torch's. */
-/* :328 near/far + :356-364 stratified depths -> nears [N], fars [N], z [N,64] */
+/* The per-ray stages of NeRFRenderer.run (external/nerf/renderer_df.py:310-468), one warp per ray, for Tc = num_steps coarse and
+ * Tf = upsample_steps importance samples per ray: num_steps >= 1, num_steps + upsample_steps <= 256 (a sorted slot index fits a uint8),
+ * num_steps >= 2 when upsample_steps > 0.  Counts outside that return SFB_ERR_ARG.  get_default_torch_ngp_opt uses 64 + 64.
+ * All random draws of the reference are inputs: noise [N,Tc] U(0,1) or NULL (perturb=False, :363); u [N,Tf] (torch.rand at :31, or the
+ * deterministic linspace of :28 in eval mode).  lin = torch.linspace(0,1,Tc) (:356), passed in so depths are bit-identical to torch's
+ * on CUDA tensors, where (far - near) / Tc is a multiplication by the fp32 reciprocal of Tc. */
+/* :328 near/far + :356-364 stratified depths -> nears [N], fars [N], z [N,Tc] */
 int sfb_ray_coarse_z(const float* rays_o, const float* rays_d, const float* aabb, float min_near, const float* lin, const float* noise,
                      uint32_t N, uint32_t num_steps, float* nears, float* fars, float* z, void* stream);
-/* :381-395 (+ sample_pdf :15-49) + :404-405: coarse weights -> inverse-CDF samples -> merged, sorted depths z_sorted [N,128] */
+/* :381-395 (+ sample_pdf :15-49) + :404-405: coarse weights -> inverse-CDF samples -> merged, sorted depths z_sorted [N,Tc+Tf]
+ * (ties: coarse first, then by index).  The pdf is over weights[1:-1] (Tc-2 bins); at Tc = 2 it has none and every importance sample
+ * is z_mid[0], as in the reference.  Tf = 0 copies the coarse depths. */
 int sfb_ray_resample(const float* z_coarse, const float* sigma_coarse, const float* nears, const float* fars, const float* u, int det,
                      uint32_t N, uint32_t num_steps, uint32_t upsample_steps, float* z_sorted, void* stream);
-/* same, also returning the 64 importance depths in draw order (z_new [N,64]) and, per sorted slot, where it came from (src_of [N,128] uint8:
- * t < 64 = coarse sample t, 64 + t = importance sample t).  With sfb_ray_gather_sorted the renderer evaluates the field once per sample:
- * coarse pass (sigma, rgb at the 64 stratified depths), importance pass (the 64 new depths), then this gather into sorted order. */
+/* same, also returning the Tf importance depths in draw order (z_new [N,Tf]) and, per sorted slot, where it came from (src_of [N,Tc+Tf]
+ * uint8: t < Tc = coarse sample t, Tc + t = importance sample t).  With sfb_ray_gather_sorted_steps the renderer evaluates the field once
+ * per sample: coarse pass (sigma, rgb at the Tc stratified depths), importance pass (the Tf new depths), then this gather into sorted order. */
 int sfb_ray_resample_ex(const float* z_coarse, const float* sigma_coarse, const float* nears, const float* fars, const float* u, int det, uint32_t N,
                         uint32_t num_steps, uint32_t upsample_steps, float* z_sorted, float* z_new, uint8_t* src_of, void* stream);
+/* sigma [N,Tc+Tf], rgb [N,Tc+Tf,3] in sorted order from the coarse pass (sigma_coarse [N,Tc], rgb_coarse [N,Tc,3]) and the importance
+ * pass (sigma_new [N,Tf], rgb_new [N,Tf,3]; may be NULL when Tf = 0) through src_of */
+int sfb_ray_gather_sorted_steps(const uint8_t* src_of, const float* sigma_coarse, const float* rgb_coarse, const float* sigma_new, const float* rgb_new,
+                                uint32_t N, uint32_t num_steps, uint32_t upsample_steps, float* sigma, float* rgb, void* stream);
+/* the 64 + 64 case of sfb_ray_gather_sorted_steps: T must be 128 */
 int sfb_ray_gather_sorted(const uint8_t* src_of, const float* sigma_coarse, const float* rgb_coarse, const float* sigma_new, const float* rgb_new,
                           uint32_t N, uint32_t T, float* sigma, float* rgb, void* stream);
-/* :414-456: weights = alpha * cumprod(1 - alpha + 1e-15); image [N,3] (+ (1-ws)*bg_color), depth [N], weights_sum [N] */
+/* :414-456 over T = Tc + Tf sorted samples, the last delta (far - near) / Tc: weights = alpha * cumprod(1 - alpha + 1e-15);
+ * image [N,3] (+ (1-ws)*bg_color), depth [N], weights_sum [N].  Rays with near = far (missed) get depth 0. */
+int sfb_ray_composite_forward_steps(const float* z_sorted, const float* sigma, const float* rgb, const float* nears, const float* fars,
+                                    float bg_color, uint32_t N, uint32_t num_steps, uint32_t upsample_steps, float* image, float* depth,
+                                    float* weights_sum, void* stream);
+/* the 64 + 64 case of sfb_ray_composite_forward_steps: T must be 128 */
 int sfb_ray_composite_forward(const float* z_sorted, const float* sigma, const float* rgb, const float* nears, const float* fars,
                               float bg_color, uint32_t N, uint32_t T, float* image, float* depth, float* weights_sum, void* stream);
-/* what autograd derives for :414-456: grad_sigma [N,128], grad_rgb [N,128,3] from grad_image [N,3], grad_weights_sum / grad_depth [N] or NULL */
+/* what autograd derives for :414-456: grad_sigma [N,Tc+Tf], grad_rgb [N,Tc+Tf,3] from grad_image [N,3], grad_weights_sum / grad_depth [N]
+ * or NULL; zero for missed rays */
+int sfb_ray_composite_backward_steps(const float* z_sorted, const float* sigma, const float* rgb, const float* nears, const float* fars,
+                                     float bg_color, uint32_t N, uint32_t num_steps, uint32_t upsample_steps, const float* grad_image,
+                                     const float* grad_weights_sum, const float* grad_depth, float* grad_sigma, float* grad_rgb, void* stream);
+/* the 64 + 64 case of sfb_ray_composite_backward_steps: T must be 128 */
 int sfb_ray_composite_backward(const float* z_sorted, const float* sigma, const float* rgb, const float* nears, const float* fars,
                                float bg_color, uint32_t N, uint32_t T, const float* grad_image, const float* grad_weights_sum,
                                const float* grad_depth, float* grad_sigma, float* grad_rgb, void* stream);

@@ -15,9 +15,10 @@ kernel (network_grid.py), and return the reference's loss_orient / loss_smooth.
 
 ``run`` is the default path (opt.cuda_ray = False, distillation.py:505).  The reference spells it as ~150 eager
 launches and evaluates the field three times (coarse, fine, colour); here it is seven kernels and every point is
-evaluated once per role (coarse density for the sampling pdf, then sigma+rgb at the 128 sorted samples), with an
-analytic backward -- gradients equal the reference's because its fine/colour passes see the same points and
-parameters.
+evaluated once (sigma+rgb at the num_steps coarse and the upsample_steps importance depths, gathered into sorted
+order), with an analytic backward -- gradients equal the reference's because its fine/colour passes see the same
+points and parameters.  'albedo' renders at any num_steps >= 1, upsample_steps >= 0 with num_steps + upsample_steps
+<= 256 (num_steps >= 2 when upsample_steps > 0); the normal-based shadings at 64 + 64.
 """
 from __future__ import annotations
 
@@ -30,36 +31,40 @@ from . import _lib as lib
 from . import raymarching
 
 
-def _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
-    """renderer_df.run :328-412: near/far, the 64 stratified and 64 importance depths, and sigma, rgb at the 128 sorted samples
-    -> (zs [N,128], sigma [N,128], rgb [N,128,3], nears [N], fars [N])"""
+def _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2, num_steps=64, upsample_steps=64):
+    """renderer_df.run :328-412: near/far, the num_steps stratified and upsample_steps importance depths, and sigma, rgb at the
+    T = num_steps + upsample_steps sorted samples -> (zs [N,T], sigma [N,T], rgb [N,T,3], nears [N], fars [N]).  With upsample_steps = 0
+    these are the coarse samples themselves (the reference skips importance sampling, :372)."""
     N = rays_o.shape[0]
     dev = rays_o.device
     enc = net.encoder
     S, H, bound = float(math.log2(enc.per_level_scale)), int(enc.base_resolution), float(net.bound)
     st = lib.stream()
     f = lib.fptr
+    Tc, Tf = num_steps, upsample_steps
     nears, fars = torch.empty(N, device=dev), torch.empty(N, device=dev)
-    zc = torch.empty(N, 64, device=dev)
-    lin = torch.linspace(0.0, 1.0, 64, device=dev)
-    lib.call('sfb_ray_coarse_z', f(rays_o), f(rays_d), f(aabb), float(min_near), f(lin), f(perturb_noise), N, 64, f(nears), f(fars), f(zc), st)
-    # the field is evaluated ONCE per sample: coarse pass (sigma + rgb at the 64 stratified depths), importance pass (the 64 new depths),
+    zc = torch.empty(N, Tc, device=dev)
+    lin = torch.linspace(0.0, 1.0, Tc, device=dev)
+    lib.call('sfb_ray_coarse_z', f(rays_o), f(rays_d), f(aabb), float(min_near), f(lin), f(perturb_noise), N, Tc, f(nears), f(fars), f(zc), st)
+    # the field is evaluated ONCE per sample: coarse pass (sigma + rgb at the Tc stratified depths), importance pass (the Tf new depths),
     # then a gather into sorted order -- the values of the coarse samples are the same numbers a second evaluation would produce
-    sig_c, rgb_c = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
+    sig_c, rgb_c = torch.empty(N, Tc, device=dev), torch.empty(N, Tc, 3, device=dev)
     args = (f(emb), lib.iptr(enc.offsets), S, H, bound, f(w0), f(b0), f(w1), f(b1), f(w2), f(b2))
-    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zc), 64, N * 64, *args, f(sig_c), f(rgb_c), st)
-    zs, zn = torch.empty(N, 128, device=dev), torch.empty(N, 64, device=dev)
-    src_of = torch.empty(N, 128, dtype=torch.uint8, device=dev)
-    lib.call('sfb_ray_resample_ex', f(zc), f(sig_c), f(nears), f(fars), f(pdf_u), 0, N, 64, 64, f(zs), f(zn), src_of.data_ptr(), st)
-    sig_n, rgb_n = torch.empty(N, 64, device=dev), torch.empty(N, 64, 3, device=dev)
-    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zn), 64, N * 64, *args, f(sig_n), f(rgb_n), st)
-    sigma, rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
-    lib.call('sfb_ray_gather_sorted', src_of.data_ptr(), f(sig_c), f(rgb_c), f(sig_n), f(rgb_n), N, 128, f(sigma), f(rgb), st)
+    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zc), Tc, N * Tc, *args, f(sig_c), f(rgb_c), st)
+    if Tf == 0:
+        return zc, sig_c, rgb_c, nears, fars
+    zs, zn = torch.empty(N, Tc + Tf, device=dev), torch.empty(N, Tf, device=dev)
+    src_of = torch.empty(N, Tc + Tf, dtype=torch.uint8, device=dev)
+    lib.call('sfb_ray_resample_ex', f(zc), f(sig_c), f(nears), f(fars), f(pdf_u), 0, N, Tc, Tf, f(zs), f(zn), src_of.data_ptr(), st)
+    sig_n, rgb_n = torch.empty(N, Tf, device=dev), torch.empty(N, Tf, 3, device=dev)
+    lib.call('sfb_ngp_field_forward', None, f(rays_o), f(rays_d), f(zn), Tf, N * Tf, *args, f(sig_n), f(rgb_n), st)
+    sigma, rgb = torch.empty(N, Tc + Tf, device=dev), torch.empty(N, Tc + Tf, 3, device=dev)
+    lib.call('sfb_ray_gather_sorted_steps', src_of.data_ptr(), f(sig_c), f(rgb_c), f(sig_n), f(rgb_n), N, Tc, Tf, f(sigma), f(rgb), st)
     return zs, sigma, rgb, nears, fars
 
 
 def _field_backward_at_samples(net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0, b0, w1, b1, w2, b2):
-    """parameter gradients of <sigma, g_sigma> + <rgb, g_rgb> over the field at the [N,128] ray samples"""
+    """parameter gradients of <sigma, g_sigma> + <rgb, g_rgb> over the field at the [N,T] ray samples"""
     enc = net.encoder
     dev = rays_o.device
     f = lib.fptr
@@ -67,7 +72,7 @@ def _field_backward_at_samples(net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0,
     tape = torch.empty(lib.load().sfb_ngp_field_tape_floats(B), device=dev)
     g_emb = torch.zeros_like(emb)
     gw0, gb0, gw1, gb1, gw2, gb2 = (torch.zeros_like(t) for t in (w0, b0, w1, b1, w2, b2))
-    lib.call('sfb_ngp_field_backward', None, f(rays_o), f(rays_d), f(zs), 128, B, f(emb), lib.iptr(enc.offsets), float(math.log2(enc.per_level_scale)),
+    lib.call('sfb_ngp_field_backward', None, f(rays_o), f(rays_d), f(zs), zs.shape[1], B, f(emb), lib.iptr(enc.offsets), float(math.log2(enc.per_level_scale)),
              int(enc.base_resolution), float(net.bound), f(w0), f(b0), f(w1), f(b1), f(w2), f(b2), f(g_sigma), None if g_rgb is None else f(g_rgb),
              f(g_emb), f(gw0), f(gb0), f(gw1), f(gb1), f(gw2), f(gb2), f(tape), lib.stream())
     return g_emb, gw0, gb0, gw1, gb1, gw2, gb2
@@ -77,36 +82,38 @@ class _RunRender(torch.autograd.Function):
     """renderer_df.run (:310-468) for shading='albedo', bg_radius == 0: returns (image [N,3], depth [N], weights_sum [N], nears, fars)"""
 
     @staticmethod
-    def forward(ctx, net, rays_o, rays_d, aabb, min_near, bg_color, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
+    def forward(ctx, net, rays_o, rays_d, aabb, min_near, bg_color, num_steps, upsample_steps, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2):
         N = rays_o.shape[0]
         dev = rays_o.device
         f = lib.fptr
-        zs, sigma, rgb, nears, fars = _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2)
+        zs, sigma, rgb, nears, fars = _sorted_samples(net, rays_o, rays_d, aabb, min_near, perturb_noise, pdf_u, emb, w0, b0, w1, b1, w2, b2,
+                                                      num_steps, upsample_steps)
         image, depth, ws = torch.empty(N, 3, device=dev), torch.empty(N, device=dev), torch.empty(N, device=dev)
-        lib.call('sfb_ray_composite_forward', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, 128, f(image), f(depth), f(ws), lib.stream())
+        lib.call('sfb_ray_composite_forward_steps', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, num_steps, upsample_steps, f(image),
+                 f(depth), f(ws), lib.stream())
         ctx.save_for_backward(rays_o, rays_d, zs, sigma, rgb, nears, fars, emb, w0, b0, w1, b1, w2, b2)
-        ctx.net, ctx.bg = net, float(bg_color)
+        ctx.net, ctx.bg, ctx.steps = net, float(bg_color), (num_steps, upsample_steps)
         ctx.mark_non_differentiable(nears, fars)
         return image, depth, ws, nears, fars
 
     @staticmethod
     def backward(ctx, g_image, g_depth, g_ws, _gn, _gf):
         rays_o, rays_d, zs, sigma, rgb, nears, fars, emb, w0, b0, w1, b1, w2, b2 = ctx.saved_tensors
-        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws)
+        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws, *ctx.steps)
         grads = _field_backward_at_samples(ctx.net, rays_o, rays_d, zs, g_sigma, g_rgb, emb, w0, b0, w1, b1, w2, b2)
-        return (None, None, None, None, None, None, None, None, *grads)
+        return (None, None, None, None, None, None, None, None, None, None, *grads)
 
 
-def _composite_backward(zs, sigma, rgb, nears, fars, bg, g_image, g_depth, g_ws):
-    """sfb_ray_composite_backward: (dL/dsigma [N,128], dL/drgb [N,128,3])"""
-    N = zs.shape[0]
+def _composite_backward(zs, sigma, rgb, nears, fars, bg, g_image, g_depth, g_ws, num_steps, upsample_steps):
+    """sfb_ray_composite_backward_steps: (dL/dsigma [N,T], dL/drgb [N,T,3])"""
+    N, T = zs.shape
     dev = zs.device
     f = lib.fptr
     g_image = g_image.contiguous() if g_image is not None else torch.zeros(N, 3, device=dev)
-    g_sigma, g_rgb = torch.empty(N, 128, device=dev), torch.empty(N, 128, 3, device=dev)
+    g_sigma, g_rgb = torch.empty(N, T, device=dev), torch.empty(N, T, 3, device=dev)
     g_ws = None if g_ws is None else g_ws.contiguous()
     g_depth = None if g_depth is None else g_depth.contiguous()
-    lib.call('sfb_ray_composite_backward', f(zs), f(sigma), f(rgb), f(nears), f(fars), bg, N, 128, f(g_image),
+    lib.call('sfb_ray_composite_backward_steps', f(zs), f(sigma), f(rgb), f(nears), f(fars), bg, N, num_steps, upsample_steps, f(g_image),
              None if g_ws is None else f(g_ws), None if g_depth is None else f(g_depth), f(g_sigma), f(g_rgb), lib.stream())
     return g_sigma, g_rgb
 
@@ -133,25 +140,27 @@ class _RaySamples(torch.autograd.Function):
 
 
 class _Composite(torch.autograd.Function):
-    """renderer_df.py:414-456 (bg_radius == 0): (image [N,3], depth [N], weights_sum [N]) of colours rgb [N,128,3] at depths zs"""
+    """renderer_df.py:414-456 (bg_radius == 0): (image [N,3], depth [N], weights_sum [N]) of colours rgb [N,T,3] at depths zs [N,T],
+    T = num_steps + upsample_steps"""
 
     @staticmethod
-    def forward(ctx, zs, sigma, rgb, nears, fars, bg_color):
+    def forward(ctx, zs, sigma, rgb, nears, fars, bg_color, num_steps, upsample_steps):
         N = zs.shape[0]
         dev = zs.device
         f = lib.fptr
         sigma, rgb = sigma.contiguous(), rgb.contiguous()
         image, depth, ws = torch.empty(N, 3, device=dev), torch.empty(N, device=dev), torch.empty(N, device=dev)
-        lib.call('sfb_ray_composite_forward', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, 128, f(image), f(depth), f(ws), lib.stream())
+        lib.call('sfb_ray_composite_forward_steps', f(zs), f(sigma), f(rgb), f(nears), f(fars), float(bg_color), N, num_steps, upsample_steps, f(image),
+                 f(depth), f(ws), lib.stream())
         ctx.save_for_backward(zs, sigma, rgb, nears, fars)
-        ctx.bg = float(bg_color)
+        ctx.bg, ctx.steps = float(bg_color), (num_steps, upsample_steps)
         return image, depth, ws
 
     @staticmethod
     def backward(ctx, g_image, g_depth, g_ws):
         zs, sigma, rgb, nears, fars = ctx.saved_tensors
-        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws)
-        return None, g_sigma, g_rgb, None, None, None
+        g_sigma, g_rgb = _composite_backward(zs, sigma, rgb, nears, fars, ctx.bg, g_image, g_depth, g_ws, *ctx.steps)
+        return None, g_sigma, g_rgb, None, None, None, None, None
 
 
 def _safe_normalize(x, eps=1e-20):
@@ -160,7 +169,8 @@ def _safe_normalize(x, eps=1e-20):
 
 
 class NeRFRenderer(nn.Module):
-    MAX_RAYS_PER_LAUNCH = 65536      # rays per fused-render autograd node (x 128 samples x 1.4 KB of backward tape = 12 GB transient)
+    MAX_RAYS_PER_LAUNCH = 65536      # rays per fused-render autograd node at 128 samples per ray (x 1.4 KB of backward tape = 12 GB transient)
+    MAX_SAMPLES_PER_RAY = 256        # num_steps + upsample_steps: the fused kernels index a ray's sorted samples with a uint8
 
     def __init__(self, opt):
         super().__init__()
@@ -233,11 +243,19 @@ class NeRFRenderer(nn.Module):
         """rays_o, rays_d: [B, N, 3] (B == 1) -> image [B,N,3], depth [B,N], weights_sum [N], mask [B,N], and with a shading other than
         'albedo' loss_orient and loss_smooth (:427-436).  ``perturb_noise`` [N,num_steps] / ``pdf_noise`` [N,upsample_steps] /
         ``normal_noise`` [N,128,3] override the torch.rand / torch.randn draws (parity tests).  ``regularisers=False`` skips loss_orient and
-        loss_smooth (and the randn of :434 with them): ``render(staged=True)`` passes it, since the reference discards them there."""
+        loss_smooth (and the randn of :434 with them): ``render(staged=True)`` passes it, since the reference discards them there.
+        'albedo' takes num_steps >= 1 and upsample_steps >= 0 with num_steps + upsample_steps <= 256 (num_steps >= 2 when upsample_steps > 0:
+        at 1 the reference itself fails); upsample_steps = 0 composites the coarse samples alone.  The other shadings take 64 + 64."""
         if self.bg_radius > 0:
             raise NotImplementedError("the fused renderer covers SparseFusion's configuration: bg_radius=0 (sparsefusion/distillation.py:512)")
-        if num_steps != 64 or upsample_steps != 64:
-            raise NotImplementedError('the fused renderer is built for num_steps = upsample_steps = 64 (get_default_torch_ngp_opt)')
+        if shading != 'albedo' and (num_steps != 64 or upsample_steps != 64):
+            raise NotImplementedError(f"shading={shading!r} renders at num_steps = upsample_steps = 64 (get_default_torch_ngp_opt); 'albedo' takes other counts")
+        if num_steps < 1 or upsample_steps < 0 or (num_steps == 1 and upsample_steps > 0):
+            raise ValueError(f'num_steps = {num_steps}, upsample_steps = {upsample_steps}: needs num_steps >= 1, upsample_steps >= 0, and num_steps >= 2 '
+                             'when upsample_steps > 0 (the importance pdf is over the coarse bins)')
+        if num_steps + upsample_steps > self.MAX_SAMPLES_PER_RAY:
+            raise NotImplementedError(f'num_steps + upsample_steps = {num_steps + upsample_steps}: the fused renderer takes at most '
+                                      f'{self.MAX_SAMPLES_PER_RAY} samples per ray')
         prefix = rays_o.shape[:-1]
         rays_o = rays_o.contiguous().view(-1, 3).float()
         rays_d = rays_d.contiguous().view(-1, 3).float()
@@ -261,24 +279,29 @@ class NeRFRenderer(nn.Module):
                 perturb_noise = torch.rand(N, num_steps, device=dev)                          # renderer_df.py:363
             if not perturb:
                 perturb_noise = None
-            if self.training:
+            if upsample_steps == 0:                                                            # no sample_pdf, no draw (:372)
+                pdf_u = None
+            elif self.training:
                 pdf_u = pdf_noise if pdf_noise is not None else torch.rand(N, upsample_steps, device=dev)   # renderer_df.py:31
             else:                                                                              # det = not self.training (:392)
                 pdf_u = torch.linspace(0. + 0.5 / upsample_steps, 1. - 0.5 / upsample_steps, steps=upsample_steps, device=dev).expand(N, upsample_steps)
-            pdf_u = pdf_u.contiguous()
+            pdf_u = None if pdf_u is None else pdf_u.contiguous()
             p = self._field_params()
             pn = None if perturb_noise is None else perturb_noise.contiguous()
             if shading != 'albedo':
                 return self._run_shaded(rays_o, rays_d, prefix, aabb, bg_color, pn, pdf_u, light_d, ambient_ratio, shading, normal_noise,
                                         regularisers)
-            if N <= self.MAX_RAYS_PER_LAUNCH:
-                image, depth, ws, nears, fars = _RunRender.apply(self, rays_o, rays_d, aabb, self.min_near, bg_color, pn, pdf_u, *p)
+            # large images (512x512 rays and up at 128 samples): the backward's activation tapes are 1.4 KB per sample point, so rays go through
+            # the fused kernels in slices of a fixed sample count -- each slice is its own autograd node, whose tape exists only while that slice
+            # back-propagates
+            M = self.MAX_RAYS_PER_LAUNCH * 128 // (num_steps + upsample_steps)
+            steps = (num_steps, upsample_steps)
+            if N <= M:
+                image, depth, ws, nears, fars = _RunRender.apply(self, rays_o, rays_d, aabb, self.min_near, bg_color, *steps, pn, pdf_u, *p)
             else:
-                # large images (512x512 rays and up): the backward's activation tapes are 1.4 KB per sample point, so rays go through the fused
-                # kernels in slices -- each slice is its own autograd node, whose tape exists only while that slice back-propagates
-                parts = [_RunRender.apply(self, rays_o[i:i + self.MAX_RAYS_PER_LAUNCH], rays_d[i:i + self.MAX_RAYS_PER_LAUNCH], aabb, self.min_near, bg_color,
-                                          None if pn is None else pn[i:i + self.MAX_RAYS_PER_LAUNCH], pdf_u[i:i + self.MAX_RAYS_PER_LAUNCH], *p)
-                         for i in range(0, N, self.MAX_RAYS_PER_LAUNCH)]
+                parts = [_RunRender.apply(self, rays_o[i:i + M], rays_d[i:i + M], aabb, self.min_near, bg_color, *steps, None if pn is None else pn[i:i + M],
+                                          None if pdf_u is None else pdf_u[i:i + M], *p)
+                         for i in range(0, N, M)]
                 image, depth, ws, nears, fars = (torch.cat([q[j] for q in parts]) for j in range(5))
         return {'image': image.view(*prefix, 3), 'depth': depth.view(*prefix), 'weights_sum': ws, 'mask': (nears < fars).reshape(*prefix)}
 
@@ -312,7 +335,7 @@ class NeRFRenderer(nn.Module):
         else:
             normal = _NormalFn.apply(self, None, rays, 1e-2, True, *p)
         color, _ = shade(albedo.view(-1, 3), normal, light_d, ratio, shading)
-        image, depth, ws = _Composite.apply(zs, sigma, color.view(N, 128, 3), nears, fars, bg_color)
+        image, depth, ws = _Composite.apply(zs, sigma, color.view(N, 128, 3), nears, fars, bg_color, 64, 64)
         if not regularisers:
             return image, depth, ws, nears, fars
         with torch.no_grad():
