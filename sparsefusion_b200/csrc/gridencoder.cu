@@ -266,10 +266,14 @@ int sfb_grid_corner_rows(const float* inputs, const int32_t* offsets, int32_t* r
     SFB_REQUIRE(inputs && offsets && rows, "grid_corner_rows: null pointer");
     dim3 grid(ceil_div(B, 256u), L);
     cudaStream_t st = as_stream(stream);
+    // every D the encoder accepts, so that the rows of each instantiation can be checked
     switch (D) {
+        case 1: grid_rows_kernel<1><<<grid, 256, 0, st>>>(inputs, offsets, rows, B, L, S, H, gridtype, align_corners != 0); break;
         case 2: grid_rows_kernel<2><<<grid, 256, 0, st>>>(inputs, offsets, rows, B, L, S, H, gridtype, align_corners != 0); break;
         case 3: grid_rows_kernel<3><<<grid, 256, 0, st>>>(inputs, offsets, rows, B, L, S, H, gridtype, align_corners != 0); break;
-        default: return fail(SFB_ERR_ARG, "grid_corner_rows: D must be 2 or 3");
+        case 4: grid_rows_kernel<4><<<grid, 256, 0, st>>>(inputs, offsets, rows, B, L, S, H, gridtype, align_corners != 0); break;
+        case 5: grid_rows_kernel<5><<<grid, 256, 0, st>>>(inputs, offsets, rows, B, L, S, H, gridtype, align_corners != 0); break;
+        default: return fail(SFB_ERR_ARG, "grid_corner_rows: D must be 1..5");
     }
     return check_launch("grid_corner_rows");
 }
