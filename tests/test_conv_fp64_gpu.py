@@ -13,8 +13,8 @@ Operands sit inside NaN-filled buffers: the channels between a slice and its row
 so a tensor map that reads past Cin, Cout, the last image or a slice shows up as NaN; output channels outside the slice must stay
 bit-identical.  The tracer names every replayed launch, and ``launch_plan`` must name the same kernel.
 
-Out of scope: ordering hazards between launches (isolated replays cannot see them), the LPIPS head and prep kernels, and the NGP
-weight-gradient GEMMs issued from C (tests/test_ngp_field_fp64_gpu.py)."""
+Out of scope: ordering hazards between launches, which isolated replays cannot see (tests/test_insitu_fp64_gpu.py checks every launch in
+place), the LPIPS head and prep kernels, and the NGP weight-gradient GEMMs issued from C (tests/test_ngp_field_fp64_gpu.py)."""
 import ctypes
 import math
 import os

@@ -13,7 +13,7 @@ stay bit-identical.  The tracer names the kernels that ran; they must equal ``ke
 must agree bit for bit.
 
 Out of scope: GEMMs (tests/test_conv_fp64_gpu.py), the sampler updates, image_glue.cu and the EFT-only kernels of eft_ops.cu
-(tests/test_step_fp64_gpu.py) and ordering hazards between launches."""
+(tests/test_step_fp64_gpu.py) and ordering hazards between launches (tests/test_insitu_fp64_gpu.py checks every launch in place)."""
 import ctypes
 import math
 from collections import defaultdict
