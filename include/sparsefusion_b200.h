@@ -258,6 +258,20 @@ int sfb_plms_update_rows_cfg(const float* x, const float* e_cond, const float* e
                              const float* e3, float c0, float c1, float c2, float c3, const float* noise, const float* row_scalars, float clip,
                              float* x_prev, float* e_out, int rows, int64_t row_len, void* stream);
 
+/* DDPM.forward_noloss (sparsefusion/vldm.py:632-709, the one-step target) for `rows` contiguous rows of row_len floats (rows <= 65535), each
+ * at its own noise level: log_snr [rows] is the DEVICE array of the rows' fp32 log-SNR (alpha_cosine_log_snr of their times, evaluated by
+ * torch, the value the UNet is conditioned on), so nothing is read back to the host.  alpha = sqrt(sigmoid(ls)), sigma = sqrt(sigmoid(-ls)).
+ * Products, sums and quotients are rounded one by one, as torch evaluates these expressions.
+ * q_sample (imagen_pytorch.py:260-269): x_noisy = alpha*x_start + sigma*noise;  alpha_cumprod [rows] (may be NULL) = sigmoid(ls). */
+int sfb_ddpm_q_sample_rows(const float* x_start, const float* noise, const float* log_snr, int rows, int64_t row_len, float* x_noisy,
+                           float* alpha_cumprod, void* stream);
+/* predict_start_from_noise + clamp (imagen_pytorch.py:293-297, vldm.py:700-701): eps = e_cond, or with e_null given (classifier-free
+ * guidance: e_cond / e_null are the conditional and null halves of one batch-2*rows UNet evaluation)
+ *   eps = e_null + (e_cond - e_null) * cond_scale   (rounded without contraction, as sfb_plms_update_rows_cfg);
+ * eps_out (may be NULL) receives eps;  x0_out = clamp((x_noisy - sigma*eps) / max(alpha, 1e-8), +-clip), keeping NaN as torch.clamp does. */
+int sfb_ddpm_predict_x0_rows(const float* x_noisy, const float* e_cond, const float* e_null, float cond_scale, const float* log_snr, float clip,
+                             int rows, int64_t row_len, float* eps_out, float* x0_out, void* stream);
+
 /* One step of DDPM.p_sample with dynamic thresholding (sparsefusion/vldm.py:289-361), B rows of row_len floats (row_len <= 65536):
  *   e = cond_scale*e_cond + (1-cond_scale)*e_null (e_null may be NULL: e = e_cond);  x0 = (x - sigma*e) / max(alpha,1e-8);
  *   s = max(torch.quantile(|x0|, percentile, 'linear'), 1) per row, computed exactly;  x0 = clamp(x0, +-s) / s;

@@ -27,6 +27,9 @@ Two step semantics:
 * ``MultiSceneDistiller`` / ``distill_scenes`` distil S scenes at once, each on the reference's iteration exactly; only the SDS sub-step's VAE
   encode, PLMS sampling (``PLMSSampler.sample_rows``: every scene at its own noise level) and decode are batched over the scenes.
 
+Every entry point takes ``sds_method``: 'plms' (default) samples the SDS target with the reference's multi-step PLMS run, 'onestep' with
+``DDPM.forward_noloss`` -- one UNet evaluation per target at the same noise level (see ``Distiller``).
+
 ``fusion_substep`` / ``photometric_substep`` with world_size > 1 remain as the one-view-per-rank form (rank r takes entry 1 + r of the
 permutation, all-reduce, Adam with grad_scale 1/R) that ``tests/test_multirank_gpu.py`` pins against the single-rank minibatch.
 """
@@ -42,6 +45,7 @@ import torch.nn.functional as F
 from . import _lib as lib
 from . import image_glue as glue
 from .plms import PLMSSampler, _log_snr as plms_log_snr, _sigmoid as plms_sigmoid, check_cond_scale
+from .vldm import keep_mask
 
 
 def _check_cond_scale(vldm, cond_scale, where):
@@ -50,6 +54,16 @@ def _check_cond_scale(vldm, cond_scale, where):
     if not math.isfinite(float(cond_scale)):
         raise ValueError(f'{where}: cond_scale must be finite (got {cond_scale!r})')
     check_cond_scale(vldm, cond_scale, where)
+
+
+SDS_METHODS = ('plms', 'onestep')
+
+
+def _check_sds_method(sds_method, where):
+    """ValueError, before any device work, for an SDS target method other than 'plms' (the reference's multi-step PLMS run) and 'onestep'
+    (``DDPM.forward_noloss``)"""
+    if sds_method not in SDS_METHODS:
+        raise ValueError(f'{where}: sds_method must be one of {SDS_METHODS} (got {sds_method!r})')
 
 
 def normalize(x):  # utils/common_utils.py:9-13
@@ -198,11 +212,23 @@ class FlatAdam:
 
 
 class Distiller:
+    """One scene's distillation loop body (see the module docstring for the step semantics).
+
+    ``sds_method`` picks the SDS target of each view's VAE latent.  'plms' (the default, the reference's): the multi-step PLMS run from
+    ``max_thres`` (``PLMSSampler``, about 38 UNet evaluations on average).  'onestep': ``DDPM.forward_noloss`` at the step's own noise
+    level -- times = the ``max_thres`` PLMS would start from, so both methods use the same levels and the same fusion weight
+    1 - alpha_cumprod -- ONE UNet evaluation per target (a graph replay of the chunk's B rows, 2B guided), then the same decode, loss,
+    LPIPS and Adam.  ``cond_scale`` guides either target.  Draws of the one-step target: torch's global generator in ``step`` (the
+    reference's order: noise, then the conditional-dropout keep mask); in ``minibatch_step`` (and in ``MultiSceneDistiller``'s scenes) each
+    view's noise, then its keep uniform, from its own ``view_seed(seed, itr, view, 2)`` generator, so a view's target does not depend on its
+    batch-mates.  An unknown ``sds_method`` raises ValueError before any device work."""
+
     def __init__(self, ngp, vae, vldm, opt, cache: SceneCache, *, z_scale_factor=0.18215, plms_steps=50, start_fusion_step=1000,
                  lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3, seed=0, rank=0, world_size=1, process_group=None,
                  use_cuda_graph=True, fused_glue=True, percep=None, lambda_percep=0.1, start_percep_step=1000, views_per_step=None, max_batch=32,
-                 cond_scale=1.0):
+                 cond_scale=1.0, sds_method='plms'):
         _check_cond_scale(vldm, cond_scale, 'Distiller')
+        _check_sds_method(sds_method, 'Distiller')
         self.ngp, self.vae, self.vldm, self.opt, self.cache = ngp, vae, vldm, opt, cache
         self.z_scale_factor = z_scale_factor
         self.start_fusion_step = start_fusion_step
@@ -213,6 +239,7 @@ class Distiller:
         self.max_batch = max_batch     # views per VAE / PLMS batch on one rank (activations of the VAE decoder: 0.27 GB per tensor per 8 views at 256^2)
         # classifier-free guidance scale of the SDS target's PLMS run (1: none); with guidance the UNet evaluates 2 rows per view
         self.cond_scale = float(cond_scale)
+        self.sds_method = sds_method   # SDS target: 'plms' (multi-step PLMS run) or 'onestep' (DDPM.forward_noloss, one UNet evaluation)
         self.seed = seed
         # perceptual term (distillation.py:161, :176-178, :312-314): a PerceptualLoss module (lpips_vgg.py) or None; lambda switches on at start_percep_step
         self.percep, self.lambda_percep, self.start_percep_step = percep, lambda_percep, start_percep_step
@@ -320,7 +347,7 @@ class Distiller:
             fusion_loss = (fusion_weight * (image - pred_img).abs().mean()).sum()             # :310 ([1]-shaped in the reference)
             if self.percep is not None and itr >= self.start_percep_step:                     # :176-178, :312-314
                 fusion_loss = fusion_loss + self.percep(image, pred_img, normalize=True).mean() * self.lambda_percep
-            self.last['unet_calls'] = self.sampler.last_unet_calls
+            self._note_target_calls()
         else:                                                                                 # EFT bootstrap :316-329
             noisy_rgb = c.target_eft_image[vi:vi + 1]
             noisy_mask = (noisy_rgb.mean(dim=1, keepdim=True) > .1).float()                   # :269-271
@@ -341,7 +368,7 @@ class Distiller:
         self.last['fusion_loss'] = loss
         return loss
 
-    def _fusion_views(self, itr, views, feats, max_thres, keyed, scale):
+    def _fusion_views(self, itr, views, feats, max_thres, keyed, scale, first=True):
         """fusion term of target views ``views`` (conditioning ``feats``, read in the SDS phase only) with the image-space work in three kernels
         (bilinear x2 to NCHW for the VAE, loss value + gradient at full resolution, adjoint of the bilinear back to the render's [N,3] / [N]
         outputs): renders, ONE SDS target batch passed through ``pred_img_hook`` (or the EFT bootstrap), each view's gradient scaled by
@@ -350,14 +377,16 @@ class Distiller:
         renders = self._fusion_renders(itr, views, keyed)
         pred = [None] * len(views)
         if itr > self.start_fusion_step:                                                      # :294
-            noise_fn = None
-            if keyed:
+            noise_fn = seeds = None
+            if keyed and self.sds_method == 'onestep':
+                seeds = [view_seed(self.seed, itr, v, 2) for v in views]
+            elif keyed:
                 noise_fn = self.plms_noise(views) if self.plms_noise is not None else KeyedNoise([view_seed(self.seed, itr, v, 2) for v in views],
                                                                                                  renders[0][0].device)
-            pred = self._fusion_target([r[3] for r in renders], feats, max_thres, noise_fn)[0]
+            pred = self._fusion_target([r[3] for r in renders], feats, max_thres, noise_fn, seeds=seeds)[0]
             if self.pred_img_hook is not None:
                 pred = self.pred_img_hook(views, pred)
-            self.last['unet_calls'] = self.sampler.last_unet_calls
+            self._note_target_calls(first)
         return [self._fusion_grad(itr, *r, v, p, max_thres, scale) for r, v, p in zip(renders, views, pred)]
 
     def _fusion_renders(self, itr, views, keyed):
@@ -367,16 +396,54 @@ class Distiller:
         renders = [self._render(c.target_rays_o[v], c.target_rays_d[v], self._render_draws(c.target_rays_o[v], itr, v, 1, keyed)) for v in views]
         return [(img, ws, hw, glue.upsample2x_render(img.detach(), ws.detach(), hw, hw)) for img, ws, hw in renders]
 
+    def _note_target_calls(self, first=True):
+        """``last['unet_calls']`` of the SDS target batch just made: the PLMS run's evaluations, or 1 for the one-step target, whose graph
+        replays of the sub-step (one per batch; ``first``: the sub-step's first batch) ``last['graph_replays']`` counts"""
+        if self.sds_method == 'onestep':
+            self.last['unet_calls'] = 1
+            self.last['graph_replays'] = 1 if first else self.last.get('graph_replays', 0) + 1
+        else:
+            self.last['unet_calls'] = self.sampler.last_unet_calls
+
     @torch.no_grad()
-    def _fusion_target(self, images, feats, max_thres, noise_fn, sampler=None):
+    def _onestep_target(self, latents, max_thres, feats, seeds):
+        """``DDPM.forward_noloss`` of the B latents at times = ``max_thres`` (one float, or one per row): ONE UNet evaluation of the batch
+        (2B rows guided).  ``seeds``: per row, the generator of its noise and then its keep uniform; None: torch's global generator, in the
+        reference's order.  Returns what ``PLMSSampler.sample`` returns: (pred_x0, x_noisy, noise, alpha_cumprod)."""
+        b, dev = latents.shape[0], latents.device
+        mts = [float(m) for m in max_thres] if isinstance(max_thres, (list, tuple)) else [float(max_thres)] * b
+        times = torch.tensor(mts, dtype=torch.float32).to(dev)
+        noise = keep = None
+        if seeds is not None:
+            prob = 1 - self.vldm.cond_drop_prob
+            draw_u = self.cond_scale == 1 and prob not in (0, 1)
+            noise, u = [], []
+            for sd in seeds:
+                g = torch.Generator(device=dev)
+                g.manual_seed(int(sd))
+                noise.append(torch.randn(latents.shape[1:], generator=g, device=dev))
+                if draw_u:
+                    u.append(torch.rand(1, generator=g, device=dev))
+            noise = torch.stack(noise)
+            if self.cond_scale == 1:
+                keep = keep_mask(torch.cat(u) if draw_u else None, prob, b, dev)
+        _, x0, x_noisy, noise, acp = self.vldm.forward_noloss(latents, cond_images=feats, return_noise=True, times=times, noise=noise, keep=keep,
+                                                              cond_scale=self.cond_scale)
+        return self.vldm.unnormalize_img(x0), x_noisy, noise, acp
+
+    @torch.no_grad()
+    def _fusion_target(self, images, feats, max_thres, noise_fn, sampler=None, seeds=None):
         """the denoised targets of a batch of renders ([C>=3,H,W] each, colour first): VAE encode (:299), PLMS sampling (:304), decode (:309).
         Returns (pred_img [B,3,H,W], alpha_cumprod [B] of the run's first noise level, fp32).  ``max_thres`` is one float shared by the batch
         (``PLMSSampler.sample``) or one per row (``PLMSSampler.sample_rows``); ``noise_fn`` serves the run's draws, None: the sampler's own.
-        The run is guided with ``self.cond_scale``."""
+        The run is guided with ``self.cond_scale``.  With ``sds_method='onestep'`` the sampling is ``_onestep_target`` at the same levels, its
+        draws from the per-row generators of ``seeds`` (None: torch's global generator)."""
         sampler = self.sampler if sampler is None else sampler
         batch = images[0][None, :3] if len(images) == 1 else torch.stack([im[:3] for im in images])
         latents = self.vae.encode(normalize(batch)).mode() * self.z_scale_factor                # :299
-        if isinstance(max_thres, (list, tuple)):
+        if self.sds_method == 'onestep':
+            out = self._onestep_target(latents, max_thres, feats, seeds)
+        elif isinstance(max_thres, (list, tuple)):
             out = sampler.sample_rows(latents, max_thres, feats, noise_fn=noise_fn, cond_scale=self.cond_scale)
         else:
             prev = sampler.noise_fn
@@ -452,7 +519,7 @@ class Distiller:
         for lo in range(0, len(mine), self.max_batch):
             chunk = mine[lo:lo + self.max_batch]
             feats = c.target_features[chunk] if sds else None         # cache fields take int, one-row slice or list indices (bench.py's staged cache)
-            for lv in self._fusion_views(itr, chunk, feats, max_thres, True, inv_v):
+            for lv in self._fusion_views(itr, chunk, feats, max_thres, True, inv_v, first=lo == 0):
                 loss_b = loss_b + lv * inv_v
         self.optimizer.sync_grads(R, self.pg)              # the step's ONE collective: sum of every rank's (photometric + fusion) gradient
         self.optimizer.step(grad_scale=1.0)
@@ -472,6 +539,11 @@ class MultiSceneDistiller:
     (each scene at its own noise level, so with its own number of UNet evaluations; the UNet runs at the batch of scenes still sampling) and
     ONE decode, in chunks of at most ``max_batch`` scenes.  The SDS phase's UNet and VAE run at batch S instead of S times at batch 1.
 
+    ``sds_method`` ('plms' or 'onestep', see ``Distiller``) is every scene's SDS target.  With 'onestep' a chunk's targets are ONE
+    ``DDPM.forward_noloss`` call -- one graph replay of its b scenes (2b guided), each at its own level, one UNet evaluation per scene --
+    whose draws come from each scene's ``view_seed(seeds[k], itr, v, 2)`` generator (noise, then the keep uniform); ``plms_noise`` is not
+    used.
+
     ``cond_scale`` guides every scene's SDS target with the same classifier-free guidance scale (1: none; ValueError at construction when the
     VLDM has no conditional dropout).  ``max_batch`` counts scenes, guided or not: a guided chunk of b scenes still sampling evaluates its
     conditional and null rows as one UNet batch of 2b rows, so the sampler's CUDA graphs cover the batch sizes 1..max_batch unguided and
@@ -486,8 +558,9 @@ class MultiSceneDistiller:
     Not supported: ``views_per_step`` (NotImplementedError), ``fused_glue=False`` and ``opt.hw_scale != 2`` (NotImplementedError), scenes of
     different image, latent or ray sizes (ValueError), CPU tensors (RuntimeError)."""
 
-    def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, cond_scale=1.0, **kw):
+    def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, cond_scale=1.0, sds_method='plms', **kw):
         _check_cond_scale(vldm, cond_scale, 'MultiSceneDistiller')
+        _check_sds_method(sds_method, 'MultiSceneDistiller')
         if kw.get('views_per_step') is not None:
             raise NotImplementedError('MultiSceneDistiller runs the reference iteration (one target view per scene); views_per_step is not supported')
         if not kw.get('fused_glue', True) or int(opt.hw_scale) != 2:
@@ -505,13 +578,14 @@ class MultiSceneDistiller:
                 if tuple(t.shape[1:]) != tuple(getattr(caches[0], f).shape[1:]):
                     raise ValueError(f'MultiSceneDistiller: scenes differ in SceneCache.{f} size ({tuple(t.shape[1:])} vs '
                                      f'{tuple(getattr(caches[0], f).shape[1:])}); batched scenes need equal image, latent and ray sizes')
-        self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, cond_scale=cond_scale, **kw)
+        self.scenes = [Distiller(ngp, vae, vldm, opt, cache, seed=int(sd), percep=percep, cond_scale=cond_scale, sds_method=sds_method, **kw)
                        for ngp, cache, sd in zip(ngps, caches, seeds)]
         for d in self.scenes:
             d._keyed = True
         self.seeds = [int(s) for s in seeds]
         self.max_batch = int(max_batch)
         self.cond_scale = float(cond_scale)
+        self.sds_method = sds_method
         lead = self.scenes[0]
         self.start_fusion_step = lead.start_fusion_step
         # one sampler for all scenes: its UnetGraph holds one graph per UNet batch size (at most max_batch of them: see the class docstring)
@@ -568,7 +642,14 @@ class MultiSceneDistiller:
                 mts.append(float(max_thres) if max_thres is not None else u.clamp(min=0.0, max=0.99).item())
                 renders += d._fusion_renders(itr, [vi], True)
             pred = [None] * len(ks)
-            if sds:
+            if sds and self.sds_method == 'onestep':                                           # one forward_noloss of the chunk's scenes
+                feats = torch.cat([self.scenes[k].cache.target_features[v:v + 1] for k, v in zip(ks, views)])
+                pred = self.scenes[ks[0]]._fusion_target([r[3] for r in renders], feats, mts, None,
+                                                         seeds=[view_seed(self.seeds[k], itr, v, 2) for k, v in zip(ks, views)])[0]
+                replays += 1
+                for k in ks:
+                    calls[k] = self.scenes[k].last['unet_calls'] = 1
+            elif sds:
                 feats = torch.cat([self.scenes[k].cache.target_features[v:v + 1] for k, v in zip(ks, views)])
                 pred = self.scenes[ks[0]]._fusion_target([r[3] for r in renders], feats, mts, self._plms_noise_fn(ks, views, itr, renders[0][0].device),
                                                          sampler=self.sampler)[0]
@@ -763,7 +844,7 @@ class NativeSceneBuilder:
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
                       process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                      cond_scale=1.0):
+                      cond_scale=1.0, sds_method='plms'):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -801,8 +882,13 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     eps = null + (cond - null) * cond_scale, the conditional and null branches as one UNet batch (1, the default, is the reference's unguided
     loop).  It is independent of ``vldm_cond_scale``, which only guides the VLDM baseline's samples.  Guidance needs a VLDM trained with
     conditional dropout (ValueError before any work otherwise); with ``use_diffusion=False`` there is no SDS target and it is ignored.
+
+    ``sds_method`` is the SDS target (``Distiller``): 'plms', the default, is the reference's multi-step PLMS run; 'onestep' is
+    ``DDPM.forward_noloss`` at the same noise level, one UNet evaluation per target instead of about 38 -- the paper's one-step ablation
+    and a much cheaper distillation.  Any other value raises ValueError before any work.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
+    _check_sds_method(sds_method, 'distillation_loop')
     if use_diffusion:
         _check_cond_scale(vldm, cond_scale, 'distillation_loop')
     rank, world = 0, 1
@@ -812,7 +898,7 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     def make(ngps, caches, percep, seed):
         return Distiller(ngps[0], vae, vldm, opt, caches[0], plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0,   # :148-160
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
-                         start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0)
+                         start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
                                      visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
@@ -822,7 +908,7 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
                    evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                   cond_scale=1.0):
+                   cond_scale=1.0, sds_method='plms'):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -834,16 +920,18 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     ``visualize`` / ``visualize_shadings``: each scene's EFT grid, gifs and jpegs as ``distillation_loop(visualize=True)`` writes them, jitter
     keyed by ``seed + k``.  ``evaluate_baselines`` / ``vldm_cond_scale``: each scene's EFT and VLDM baselines scored and written as
     ``distillation_loop(evaluate_baselines=True)`` does, scene k's VLDM draws keyed by ``seed + k``.  ``cond_scale``: the guidance scale of
-    every scene's SDS targets, as ``distillation_loop(cond_scale=...)``, independent of ``vldm_cond_scale``.
+    every scene's SDS targets, as ``distillation_loop(cond_scale=...)``, independent of ``vldm_cond_scale``.  ``sds_method``: every scene's
+    SDS target, 'plms' or 'onestep', as ``distillation_loop(sds_method=...)``; a chunk's one-step targets are one ``forward_noloss`` call.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
+    _check_sds_method(sds_method, 'distill_scenes')
     if use_diffusion:
         _check_cond_scale(vldm, cond_scale, 'distill_scenes')
 
     def make(ngps, caches, percep, base):
         return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
-                                   lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0)
+                                   lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
                              loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
 
