@@ -552,6 +552,15 @@ int sfb_mesh_texel_points(const float* verts, const int32_t* tris, int F, int T,
  * [0, 1], as sfb_ngp_field_forward writes it. */
 int sfb_mesh_texture_pack(const int32_t* owner, const float* rgb, int64_t n, uint8_t* out, void* stream);
 
+/* ==========================================================================================
+ * section 13 -- digest of a device buffer (the scene-cache check of a resumed distillation: sparsefusion_b200/distillation.py
+ *    cache_digest; the reference has no checkpoint of its distillation loop)
+ * ========================================================================================== */
+/* out [1] uint64 <- sum over i < n_words of mix(w[i] ^ mix(i + 0x9E3779B97F4A7C15)) modulo 2^64, w = data as uint32 words, mix = splitmix64's
+ * finaliser (x ^= x >> 30; x *= 0xBF58476D1CE4E5B9; x ^= x >> 27; x *= 0x94D049BB133111EB; x ^= x >> 31).  Independent of launch geometry
+ * and atomic order.  out is zeroed on `stream` first; data may be NULL when n_words = 0. */
+int sfb_digest_u32(const void* data, int64_t n_words, uint64_t* out, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -32,10 +32,16 @@ Every entry point takes ``sds_method``: 'plms' (default) samples the SDS target 
 
 ``fusion_substep`` / ``photometric_substep`` with world_size > 1 remain as the one-view-per-rank form (rank r takes entry 1 + r of the
 permutation, all-reduce, Adam with grad_scale 1/R) that ``tests/test_multirank_gpu.py`` pins against the single-rank minibatch.
+
+Checkpoints: ``Distiller.state_dict`` / ``MultiSceneDistiller.state_dict`` hold everything a run needs to continue -- parameters, Adam
+moments and counts, the cuda_ray density grid and counters, the view-permutation generator, the global CPU / CUDA generators of every rank,
+the seed -- with a fingerprint of the step's settings and a digest of the scene cache, so that ``load_state_dict`` refuses a state it cannot
+continue.  The loops write them with ``checkpoint_every`` and continue from them with ``resume``.
 """
 from __future__ import annotations
 
 import math
+import os
 from dataclasses import dataclass
 from typing import Optional
 
@@ -159,6 +165,64 @@ class SceneCache:
         return SceneCache(*[getattr(self, f).pin_memory() for f in self.__dataclass_fields__])
 
 
+CHECKPOINT_VERSION = 1     # format of Distiller.state_dict; load_state_dict refuses any other
+
+
+def cache_digest(cache: SceneCache) -> dict:
+    """{field: (shape, digest)} of a scene cache, each digest a 64-bit checksum of the field's bits computed on its device
+    (``sfb_digest_u32``).  A resumed run rebuilds its cache and compares this instead of saving the cache."""
+    fields = list(SceneCache.__dataclass_fields__)
+    for f in fields:
+        t = getattr(cache, f)
+        if not t.is_cuda:
+            raise RuntimeError(f'cache_digest: SceneCache.{f} must be a CUDA tensor (the digest runs on the device)')
+        if (t.numel() * t.element_size()) % 4:
+            raise ValueError(f'cache_digest: SceneCache.{f} is not a whole number of 32-bit words')
+    sums = []
+    for f in fields:
+        t = getattr(cache, f).contiguous()
+        out = torch.empty(1, dtype=torch.int64, device=t.device)
+        with torch.cuda.device(t.device):
+            lib.call('sfb_digest_u32', t.data_ptr() if t.numel() else None, t.numel() * t.element_size() // 4, out.data_ptr(), lib.stream())
+        sums.append(out)
+    words = torch.cat([s.cpu() for s in sums]).tolist()
+    return {f: (tuple(getattr(cache, f).shape), w & 0xFFFFFFFFFFFFFFFF) for f, w in zip(fields, words)}
+
+
+def _plain(v):
+    """``v`` as plain, comparable Python values (lists for tuples, repr for anything else), for a fingerprint"""
+    if v is None or isinstance(v, (bool, int, float, str)):
+        return v
+    if isinstance(v, (list, tuple)):
+        return [_plain(x) for x in v]
+    if isinstance(v, dict):
+        return {str(k): _plain(x) for k, x in v.items()}
+    return repr(v)
+
+
+def _rng_states(device, world_size=1, process_group=None) -> list:
+    """[per rank] the global CPU generator's state and the CUDA generator's state of the rank's device (None on a CPU device); with
+    world_size > 1 gathered from every rank of the process group"""
+    mine = dict(cpu=torch.get_rng_state(), cuda=torch.cuda.get_rng_state(device) if device.type == 'cuda' else None)
+    if world_size == 1:
+        return [mine]
+    out = [None] * world_size
+    torch.distributed.all_gather_object(out, mine, group=process_group)
+    return out
+
+
+def _restore_rng(states, device, rank):
+    """restore this rank's entry of ``_rng_states`` (entry rank mod the saved world size)"""
+    st = states[rank % len(states)]
+    torch.set_rng_state(st['cpu'])
+    if st['cuda'] is not None and device.type == 'cuda':
+        torch.cuda.set_rng_state(st['cuda'], device)
+
+
+def _mismatch(what, saved, now):
+    return ValueError(f'load_state_dict: {what} differs: the checkpoint has {saved!r}, this run {now!r}; the saved state cannot be continued here')
+
+
 class FlatAdam:
     """torch.optim.Adam(ngp.get_params(lr)) + StepLR(step_size, gamma) (distillation.py:165-166) over ONE flat buffer:
     parameters, gradients and both moments are contiguous so that the gradient all-reduce is a single collective and
@@ -210,6 +274,27 @@ class FlatAdam:
     def scheduler_step(self):
         self.sched += 1
 
+    def state_dict(self) -> dict:
+        """Adam moments ``m`` / ``v`` (host copies) and the step and scheduler counts; the parameters are the network's"""
+        return dict(m=self.m.detach().to('cpu', copy=True), v=self.v.detach().to('cpu', copy=True), t=self.t, sched=self.sched,
+                    groups=[list(g) for g in self.groups])
+
+    def check_state(self, sd):
+        """ValueError when ``sd`` is not a state of an optimiser with this one's parameter groups"""
+        for k in ('m', 'v'):
+            if tuple(sd[k].shape) != tuple(self.m.shape):
+                raise _mismatch(f'optimizer.{k} size', tuple(sd[k].shape), tuple(self.m.shape))
+        if [list(g) for g in sd['groups']] != [list(g) for g in self.groups]:
+            raise _mismatch('optimizer parameter groups', sd['groups'], [list(g) for g in self.groups])
+
+    def load_state_dict(self, sd):
+        """copy ``m`` / ``v`` into the existing buffers in place -- the parameters and their .grad are views of ``flat`` / ``grad`` and
+        must stay so -- and restore the counts"""
+        self.check_state(sd)
+        self.m.copy_(sd['m'])
+        self.v.copy_(sd['v'])
+        self.t, self.sched = int(sd['t']), int(sd['sched'])
+
 
 class Distiller:
     """One scene's distillation loop body (see the module docstring for the step semantics).
@@ -255,6 +340,7 @@ class Distiller:
         self.plms_noise = None     # parity tests (minibatch step): callable(views) -> noise_fn for that batch, replacing KeyedNoise
         self.pred_img_hook = None  # parity tests (minibatch step): callable(views, pred_img) -> pred_img, e.g. to inject a fixed denoised target
         self._keyed = False        # MultiSceneDistiller: the reference step draws from the keyed generators too (``_render_draws``)
+        self.next_itr = 0          # the iteration after the last one run: what state_dict saves as ``itr``
         self.last = {}
 
     # ------------------------------------------------------------------------------------------------
@@ -323,11 +409,13 @@ class Distiller:
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))
         self.optimizer.scheduler_step()                                                       # :247
         self.last['photo_loss'] = loss
+        self.next_itr = itr + 1
         return loss
 
     def fusion_substep(self, itr: int, max_thres: Optional[float] = None):
         """distillation.py:259-352; rank r takes the (1 + r)-th entry of the step's permutation (the reference takes entry 1, :264)"""
         c = self.cache
+        self.next_itr = itr + 1
         self.optimizer.zero_grad()                                                            # :261
         n_t = c.target_features.shape[0]
         perm = torch.randperm(n_t, generator=self.gen)                                        # :263
@@ -526,7 +614,89 @@ class Distiller:
         self.optimizer.scheduler_step()                                                        # :247
         self.last['photo_loss'], self.last['fusion_loss'] = loss_a, loss_b
         self.last['views'] = mine
+        self.next_itr = itr + 1
         return loss_a, loss_b
+
+    # ------------------------------------------------------------------------------------------------ checkpoint / resume
+    def fingerprint(self, use_diffusion=True) -> dict:
+        """everything besides the parameters, optimiser state, draws and cache that decides what the next step computes; a checkpoint
+        continues only under an equal fingerprint.  ``use_diffusion``: whether the loop runs the fusion sub-step at all"""
+        return dict(opt=_plain(vars(self.opt)), views_per_step=self.views_per_step, max_batch=self.max_batch, cond_scale=self.cond_scale,
+                    sds_method=self.sds_method, use_diffusion=bool(use_diffusion), lambda_color=self.lambda_color, lambda_sil=self.lambda_sil,
+                    lambda_opacity=self.lambda_opacity, lambda_percep=self.lambda_percep, start_fusion_step=self.start_fusion_step,
+                    start_percep_step=self.start_percep_step, plms_steps=self.sampler.plms_steps, fused_glue=self.fused_glue,
+                    percep=self.percep is not None, z_scale_factor=self.z_scale_factor, keyed=self._keyed)
+
+    def _scene_state(self, itr, use_diffusion):
+        """this scene's part of a checkpoint: everything but the global generators"""
+        extra = {k: getattr(self.ngp, k) for k in ('mean_density', 'iter_density', 'mean_count', 'local_step')} if self.opt.cuda_ray else {}
+        return dict(version=CHECKPOINT_VERSION, itr=int(itr), world_size=self.world_size, seed=self.seed,
+                    fingerprint=self.fingerprint(use_diffusion), cache=cache_digest(self.cache),
+                    ngp={k: v.detach().to('cpu', copy=True) for k, v in self.ngp.state_dict().items()}, ngp_extra=extra,
+                    optimizer=self.optimizer.state_dict(), gen=self.gen.get_state())
+
+    def state_dict(self, itr: Optional[int] = None, use_diffusion=True) -> dict:
+        """everything needed to continue this run at iteration ``itr`` (default: the one after the last step run): a format version,
+        ``itr``, the world size, the seed, ``fingerprint(use_diffusion)``, the cache digest (``cache_digest``), the network's state dict
+        (with cuda_ray its density grid, bitfield and step counter) and plain counters (``ngp_extra``), the optimiser's state, the
+        permutation generator's state and ``rng``: every rank's global CPU and CUDA generator states.  Host tensors throughout.  With
+        world_size > 1 every rank must call it (the generator states are gathered); parameters and Adam state are the same on every rank."""
+        sd = self._scene_state(self.next_itr if itr is None else itr, use_diffusion)
+        sd['rng'] = _rng_states(self.cache.input_rgb.device, self.world_size, self.pg)
+        return sd
+
+    def check_state(self, sd, use_diffusion=True):
+        """ValueError naming the first field that keeps ``sd`` from being continued by this distiller; touches no device state"""
+        if sd.get('version') != CHECKPOINT_VERSION:
+            raise _mismatch('the checkpoint format version', sd.get('version'), CHECKPOINT_VERSION)
+        if sd['world_size'] != self.world_size:
+            if self.views_per_step is None:
+                raise _mismatch('world_size (the reference step and the one-view-per-rank form continue on the same ranks only)',
+                                sd['world_size'], self.world_size)
+            if self.opt.cuda_ray:
+                raise _mismatch('world_size (with cuda_ray the density grid and the CUDA generator are per rank)', sd['world_size'],
+                                self.world_size)
+        now = self.fingerprint(use_diffusion)
+        for k in sorted(set(now) | set(sd['fingerprint'])):
+            a, b = sd['fingerprint'].get(k), now.get(k)
+            if k == 'opt' and isinstance(a, dict) and isinstance(b, dict):
+                for o in sorted(set(a) | set(b)):
+                    if a.get(o) != b.get(o):
+                        raise _mismatch(f'opt.{o}', a.get(o), b.get(o))
+            elif a != b:
+                raise _mismatch(k, a, b)
+        if sd['seed'] != self.seed:
+            raise _mismatch('seed', sd['seed'], self.seed)
+        digest = cache_digest(self.cache)
+        for f in SceneCache.__dataclass_fields__:
+            if tuple(sd['cache'][f][0]) != digest[f][0]:
+                raise _mismatch(f'scene cache field {f} shape', tuple(sd['cache'][f][0]), digest[f][0])
+            if sd['cache'][f][1] != digest[f][1]:
+                raise _mismatch(f'scene cache field {f} contents (digest)', f'{sd["cache"][f][1]:016x}', f'{digest[f][1]:016x}')
+        mine = self.ngp.state_dict()
+        if set(sd['ngp']) != set(mine):
+            raise _mismatch('network state keys', sorted(sd['ngp']), sorted(mine))
+        for k, v in mine.items():
+            if tuple(sd['ngp'][k].shape) != tuple(v.shape):
+                raise _mismatch(f'ngp.{k} shape', tuple(sd['ngp'][k].shape), tuple(v.shape))
+        self.optimizer.check_state(sd['optimizer'])
+
+    def _load_scene_state(self, sd):
+        self.ngp.load_state_dict(sd['ngp'])          # copies into the existing tensors: the parameters stay views of the flat buffer
+        for k, v in sd['ngp_extra'].items():
+            setattr(self.ngp, k, v)
+        self.optimizer.load_state_dict(sd['optimizer'])
+        self.gen.set_state(sd['gen'])
+        self.next_itr = int(sd['itr'])
+
+    def load_state_dict(self, sd, use_diffusion=True):
+        """continue from ``state_dict``'s ``sd``: ``check_state`` first (ValueError before any device state is touched), then the network,
+        optimiser and generator states in place, and last this rank's global CPU / CUDA generator states -- call it immediately before the
+        first resumed step.  The view-batched step (``views_per_step``) may continue at another world size unless cuda_ray is on; rank r
+        then takes the generator states of saved rank r mod the saved world size."""
+        self.check_state(sd, use_diffusion)
+        self._load_scene_state(sd)
+        _restore_rng(sd['rng'], self.cache.input_rgb.device, self.rank)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -592,6 +762,7 @@ class MultiSceneDistiller:
         self.sampler = PLMSSampler(vldm, lead.sampler.plms_steps, use_cuda_graph=lead.sampler.use_cuda_graph)
         self.render_noise = None
         self.plms_noise = None     # parity tests: callable(scene) -> noise_fn(like) serving that scene's PLMS draws
+        self.next_itr = 0          # the iteration after the last one run
         self.last = {}
 
     def __len__(self):
@@ -621,12 +792,14 @@ class MultiSceneDistiller:
 
     def photometric_substep(self, itr: int):
         """every scene's photometric sub-step (:185-247) through ``Distiller.photometric_substep``; returns the [S] losses"""
+        self.next_itr = itr + 1
         return torch.stack([d.photometric_substep(itr) for d in self.scenes])
 
     def fusion_substep(self, itr: int, max_thres: Optional[float] = None):
         """every scene's fusion sub-step (:259-352) with the VAE encode, PLMS sampling and decode batched over chunks of scenes; returns the [S]
         losses.  ``max_thres`` forces one noise level for every scene (tests); by default scene k uses its own ``u`` (:303)."""
         S = len(self.scenes)
+        self.next_itr = itr + 1
         sds = itr > self.start_fusion_step
         losses, calls, replays = [None] * S, [0] * S, 0
         for lo in range(0, S, self.max_batch):
@@ -674,6 +847,32 @@ class MultiSceneDistiller:
             b = self.fusion_substep(itr, max_thres)
         self.last['photo_loss'], self.last['fusion_loss'] = a, b
         return a, b
+
+    def state_dict(self, itr: Optional[int] = None, use_diffusion=True) -> dict:
+        """``{'version', 'itr', 'scenes'}``: the shared iteration (default: the one after the last step run) and one ``Distiller.state_dict``
+        per scene, each holding the process's global generator states"""
+        itr = self.next_itr if itr is None else int(itr)
+        rng = _rng_states(self.scenes[0].cache.input_rgb.device)
+        return dict(version=CHECKPOINT_VERSION, itr=itr, scenes=[dict(d._scene_state(itr, use_diffusion), rng=rng) for d in self.scenes])
+
+    def load_state_dict(self, sd, use_diffusion=True):
+        """continue from ``state_dict``'s ``sd``: every scene checked first (ValueError naming the scene and the field, before any device
+        state is touched), then every scene's state loaded, then the global generators restored -- immediately before the first resumed step"""
+        if sd.get('version') != CHECKPOINT_VERSION:
+            raise _mismatch('the checkpoint format version', sd.get('version'), CHECKPOINT_VERSION)
+        if len(sd['scenes']) != len(self.scenes):
+            raise _mismatch('the number of scenes', len(sd['scenes']), len(self.scenes))
+        for k, (d, s) in enumerate(zip(self.scenes, sd['scenes'])):
+            if s['itr'] != sd['itr']:
+                raise ValueError(f'load_state_dict: scene {k} is saved at iteration {s["itr"]}, the others at {sd["itr"]}')
+            try:
+                d.check_state(s, use_diffusion)
+            except ValueError as e:
+                raise ValueError(f'scene {k}: {e}') from None
+        for d, s in zip(self.scenes, sd['scenes']):
+            d._load_scene_state(s)
+        self.next_itr = int(sd['itr'])
+        _restore_rng(sd['scenes'][0]['rng'], self.scenes[0].cache.input_rgb.device, 0)
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -844,7 +1043,7 @@ class NativeSceneBuilder:
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
                       process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                      cond_scale=1.0, sds_method='plms'):
+                      cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -886,6 +1085,17 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ``sds_method`` is the SDS target (``Distiller``): 'plms', the default, is the reference's multi-step PLMS run; 'onestep' is
     ``DDPM.forward_noloss`` at the same noise level, one UNet evaluation per target instead of about 38 -- the paper's one-step ablation
     and a much cheaper distillation.  Any other value raises ValueError before any work.
+
+    ``checkpoint_every=K`` writes ``{save_dir}/checkpoints/{seq_name}.ckpt`` (``Distiller.state_dict``: network, Adam state, counters, every
+    generator, seed, fingerprint and cache digest) after every iteration ``itr`` with ``(itr + 1) % K == 0`` and after the last one, before
+    ``on_iteration`` sees it.  Each write goes to a temporary file in the same directory, is fsynced and then renamed over the old one, so an
+    interruption mid-write keeps the previous checkpoint; with ``process_group`` rank 0 writes and every rank waits at a barrier.
+    ``resume=True`` builds the cache as a fresh run does and then, if the checkpoint exists, continues from it: the base seed is the saved one
+    (an explicit ``seed`` that differs is a ValueError), the global generators are restored right before the first resumed iteration, and
+    ``on_iteration`` sees only the iterations run.  A state the run cannot continue (other settings, cache, or world size where that matters:
+    ``Distiller.check_state``) is a ValueError.  With ``max_itr`` at or below the saved iteration no iteration runs and the outputs come from
+    the saved state, so a finished run with a checkpoint can be extended by a larger ``max_itr``; without a checkpoint the run starts fresh,
+    so an interrupted command can be re-issued unchanged.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distillation_loop')
@@ -901,14 +1111,14 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
                          start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
-                                     visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
+                                     visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale), checkpoint_every, resume)
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
                    evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                   cond_scale=1.0, sds_method='plms'):
+                   cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -922,6 +1132,9 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     ``distillation_loop(evaluate_baselines=True)`` does, scene k's VLDM draws keyed by ``seed + k``.  ``cond_scale``: the guidance scale of
     every scene's SDS targets, as ``distillation_loop(cond_scale=...)``, independent of ``vldm_cond_scale``.  ``sds_method``: every scene's
     SDS target, 'plms' or 'onestep', as ``distillation_loop(sds_method=...)``; a chunk's one-step targets are one ``forward_noloss`` call.
+    ``checkpoint_every`` / ``resume``: as ``distillation_loop``'s, one ``{save_dir}/checkpoints/{seq_name}.ckpt`` per scene (scene k's part
+    of ``MultiSceneDistiller.state_dict``).  Resuming needs a checkpoint at the same iteration for every scene of the call, or none (then
+    the call starts fresh); anything else is a ValueError naming the scenes.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distill_scenes')
@@ -933,7 +1146,8 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
-                             loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale))
+                             loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale),
+                             checkpoint_every, resume)
 
 
 def _baselines(enabled, vae, vldm, cond_scale):
@@ -994,15 +1208,75 @@ def _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circle, eft_image
         print('saved video', gif_path)
 
 
+def _atomic_save(obj, path):
+    """torch.save to ``path`` through a temporary file in the same directory, fsynced and then renamed over ``path``: an interruption
+    leaves either the old file or the new one, never a partial one"""
+    tmp = f'{path}.tmp'
+    try:
+        with open(tmp, 'wb') as f:
+            torch.save(obj, f)
+            f.flush()
+            os.fsync(f.fileno())
+        os.replace(tmp, path)
+    except BaseException:
+        if os.path.exists(tmp):
+            os.remove(tmp)
+        raise
+
+
+def _checkpoint_paths(save_dir, scenes):
+    return [f'{save_dir}/checkpoints/{sc[0]}.ckpt' for sc in scenes]
+
+
+def _read_checkpoints(paths, names, seed):
+    """the scenes' saved states for ``resume``, or None when no scene has one; ValueError when only some have one, when they are at
+    different iterations or base seeds, or when an explicit ``seed`` differs from the saved base seed"""
+    have = [os.path.exists(p) for p in paths]
+    if not any(have):
+        return None
+    if not all(have):
+        raise ValueError(f'resume: checkpoints exist for scenes {[n for n, h in zip(names, have) if h]} but not for '
+                         f'{[n for n, h in zip(names, have) if not h]}; a call resumes all its scenes or none')
+    states = [torch.load(p, map_location='cpu', weights_only=True) for p in paths]
+    itrs = {n: s['itr'] for n, s in zip(names, states)}
+    if len(set(itrs.values())) > 1:
+        raise ValueError(f'resume: the scenes\' checkpoints are at different iterations {itrs}; a call resumes scenes saved together')
+    bases = {n: s['base_seed'] for n, s in zip(names, states)}
+    if len(set(bases.values())) > 1:
+        raise ValueError(f'resume: the scenes\' checkpoints come from different runs (base seeds {bases})')
+    base = states[0]['base_seed']
+    if seed is not None and int(seed) != base:
+        raise ValueError(f'resume: seed={seed} differs from the base seed {base} the checkpoints were made with (pass seed=None or {base})')
+    return states
+
+
+def _write_checkpoints(dist, paths, itr, use_diffusion, base_seed):
+    """every scene's checkpoint at iteration ``itr`` (the next one to run); with a process group every rank takes part in gathering the
+    generator states, rank 0 writes and all ranks wait at a barrier"""
+    sd = dist.state_dict(itr, use_diffusion)
+    states = sd['scenes'] if isinstance(dist, MultiSceneDistiller) else [sd]
+    pg = getattr(dist, 'pg', None)
+    if getattr(dist, 'rank', 0) == 0:
+        os.makedirs(os.path.dirname(paths[0]), exist_ok=True)
+        for st, p in zip(states, paths):
+            _atomic_save(dict(st, base_seed=base_seed), p)
+    if pg is not None:
+        torch.distributed.barrier(group=pg)
+
+
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
-                      loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None):
+                      loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None, checkpoint_every=None, resume=False):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
-    ``max_itr`` iterations and one checkpoint per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
+    ``max_itr`` iterations and one saved network per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
     grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``); with ``baselines`` (``_baselines``), the EFT and VLDM
-    scores, metrics files and gifs after it.  Returns the networks."""
-    import os
+    scores, metrics files and gifs after it; with ``checkpoint_every`` / ``resume`` the checkpoints of ``distillation_loop``'s docstring.
+    Returns the networks."""
     from .lpips_vgg import PerceptualLoss
+    if checkpoint_every is not None and (isinstance(checkpoint_every, bool) or not isinstance(checkpoint_every, int) or checkpoint_every < 1):
+        raise ValueError(f'checkpoint_every must be a positive int or None (got {checkpoint_every!r})')
+    ckpt_paths = _checkpoint_paths(save_dir, scenes)
+    saved = _read_checkpoints(ckpt_paths, [sc[0] for sc in scenes], seed) if resume else None
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
     visualize_shadings = tuple(visualize_shadings)
     if not all(isinstance(sh, str) and sh and '/' not in sh for sh in visualize_shadings):
@@ -1045,13 +1319,23 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     with torch.cuda.device(device):
         perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
         ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
-        base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
+        if saved is not None:
+            base_seed = saved[0]['base_seed']
+        else:
+            base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
         dist = make(ngps, caches, perceptual_loss, base_seed)
-        for itr in range(max_itr):                                                                                  # :174
+        start = 0
+        if saved is not None:                  # restores the global generators too: nothing may draw between here and the first step
+            multi = isinstance(dist, MultiSceneDistiller)
+            dist.load_state_dict(dict(version=saved[0]['version'], itr=saved[0]['itr'], scenes=saved) if multi else saved[0], use_diffusion)
+            start = saved[0]['itr']
+        for itr in range(start, max_itr):                                                                           # :174
             if use_diffusion:
                 dist.step(itr)
             else:
                 dist.photometric_substep(itr)
+            if checkpoint_every is not None and ((itr + 1) % checkpoint_every == 0 or itr == max_itr - 1):
+                _write_checkpoints(dist, ckpt_paths, itr + 1, use_diffusion, base_seed)
             if on_iteration is not None:
                 on_iteration(itr, dist)
         torch.cuda.synchronize(device)
