@@ -403,6 +403,15 @@ int sfb_fusion_loss(const float* up, const float* target, int H, int W, int mode
  * before the adjoint of the bilinear up-sampling */
 int sfb_fusion_loss_ex(const float* up, const float* target, int H, int W, int mode, float weight, float lambda_color, float lambda_sil,
                        float lambda_opacity, const float* g_extra, float* sums, float* g_up, int h, int w, float* g_img, float* g_sil, void* stream);
+/* the two sub-steps' losses with the entropy regulariser (distillation.py:236-241, :338-344): + lambda_entropy * mean H(a), a = clamp(sil,
+ * 1e-5, 1 - 1e-5), H(a) = -a log2 a - (1 - a) log2 (1 - a), over the render's opacity (photometric) or the up-sampled one (fusion, its
+ * gradient through the same bilinear adjoint).  sums[4]: the three sums above and sums[3] = sum H.  d/dsil of the term is zero where the
+ * clamp moves sil (outside [1e-5, 1 - 1e-5]), as autograd's clamp backward.  Otherwise as sfb_photometric_loss / sfb_fusion_loss_ex. */
+int sfb_photometric_loss_ent(const float* img, const float* sil, const float* rgb, const float* mask, int h, int w, int scale, float lambda_color,
+                             float lambda_sil, float lambda_opacity, float lambda_entropy, float* sums, float* g_img, float* g_sil, void* stream);
+int sfb_fusion_loss_ent(const float* up, const float* target, int H, int W, int mode, float weight, float lambda_color, float lambda_sil,
+                        float lambda_opacity, float lambda_entropy, const float* g_extra, float* sums, float* g_up, int h, int w, float* g_img,
+                        float* g_sil, void* stream);
 
 /* ==========================================================================================
  * section 7 -- LPIPS-VGG perceptual term of the fusion loss (SURVEY.md section 8f row 3)

@@ -52,14 +52,28 @@ __global__ void rays_from_camera_kernel(const float* __restrict__ cam, int H, in
     }
 }
 
+// Entropy regulariser (distillation.py:236-241, :338-344): a = clamp(s, 1e-5, 1 - 1e-5), H = -a log2 a - (1 - a) log2 (1 - a).
+// Returns H and sets dH/ds = log2((1 - a) / a) inside [1e-5, 1 - 1e-5] and 0 outside, as autograd's clamp backward gives (it passes the
+// gradient at the bounds themselves).  The bounds are the fp32 values torch compares an fp32 tensor with; a NaN s gives a NaN H.
+constexpr float kEntLo = 1e-5f, kEntHi = 0.99999f;
+
+__device__ __forceinline__ float entropy_val_grad(float s, float& grad) {
+    const float a = s < kEntLo ? kEntLo : (s > kEntHi ? kEntHi : s);
+    const float l0 = log2f(a), l1 = log2f(1.f - a);
+    grad = (s >= kEntLo && s <= kEntHi) ? l1 - l0 : 0.f;
+    return -a * l0 - (1.f - a) * l1;
+}
+
 // Photometric sub-step (distillation.py:210-234): loss = lc * mean huber(img, rgb[::2]) + ls * mean huber(sil, mask[::2]) + lo * mean sqrt(sil^2 + .01)
-// sums[0..2] += (sum huber colour, sum huber silhouette, sum opacity); gradients written directly (they do not depend on the sums).
+// (kEnt: + le * mean H(sil), :236-241).  sums[0..2] += (sum huber colour, sum huber silhouette, sum opacity), kEnt: sums[3] += sum H;
+// gradients written directly (they do not depend on the sums).
+template <bool kEnt>
 __global__ void __launch_bounds__(256) photometric_loss_kernel(const float* __restrict__ img, const float* __restrict__ sil, const float* __restrict__ rgb,
                                                               const float* __restrict__ mask, int h, int w, int scale, float lc, float ls, float lo,
-                                                              float* __restrict__ sums, float* __restrict__ g_img, float* __restrict__ g_sil) {
+                                                              float le, float* __restrict__ sums, float* __restrict__ g_img, float* __restrict__ g_sil) {
     __shared__ float sh[8];
     const int n = h * w, Hf = h * scale, Wf = w * scale;
-    float s_c = 0.f, s_s = 0.f, s_o = 0.f;
+    float s_c = 0.f, s_s = 0.f, s_o = 0.f, s_e = 0.f;
     for (int i = blockIdx.x * 256 + threadIdx.x; i < n; i += gridDim.x * 256) {
         const int y = i / w, x = i - y * w;
         const int src = (y * scale) * Wf + x * scale;
@@ -76,10 +90,20 @@ __global__ void __launch_bounds__(256) photometric_loss_kernel(const float* __re
         const float op = sqrtf(sv * sv + 0.01f);
         s_o += op;
         g_img[i * 3 + 0] = gc[0]; g_img[i * 3 + 1] = gc[1]; g_img[i * 3 + 2] = gc[2];
-        g_sil[i] = ls * huber_grad(dm) / n + lo * sv / (op * n);
+        float gs = ls * huber_grad(dm) / n + lo * sv / (op * n);
+        if constexpr (kEnt) {
+            float dh;
+            s_e += entropy_val_grad(sv, dh);
+            gs += le * dh / n;
+        }
+        g_sil[i] = gs;
     }
     const float a = block_sum_256(s_c, sh), b = block_sum_256(s_s, sh), c = block_sum_256(s_o, sh);
     if (threadIdx.x == 0) { atomicAdd(sums + 0, a); atomicAdd(sums + 1, b); atomicAdd(sums + 2, c); }
+    if constexpr (kEnt) {
+        const float e = block_sum_256(s_e, sh);
+        if (threadIdx.x == 0) atomicAdd(sums + 3, e);
+    }
 }
 
 // bilinear x2 (align_corners = False) source taps of destination index d in a length-n axis: i0, i1, weight of i1
@@ -113,12 +137,14 @@ __global__ void upsample2x_render_kernel(const float* __restrict__ img, const fl
 //   mode 0 (SDS):  loss = wgt * mean |up_rgb - target| + lo * mean sqrt(up_sil^2 + .01)                  (wgt = 1 - alpha_bar)
 //   mode 1 (EFT bootstrap): loss = lc * mean huber(up_rgb, target) + ls * mean huber(up_sil, tmask) + lo * mean sqrt(up_sil^2 + .01),
 //                           tmask = (mean_c target > 0.1)                                                  (distillation.py:269-271)
-// g_up [4][H][W] receives d loss / d up; sums[0..2] += (sum colour term, sum silhouette term, sum opacity term).
+//   kEnt: + le * mean H(up_sil) in either mode (:338-344)
+// g_up [4][H][W] receives d loss / d up; sums[0..2] += (sum colour term, sum silhouette term, sum opacity term), kEnt: sums[3] += sum H.
+template <bool kEnt>
 __global__ void __launch_bounds__(256) fusion_loss_kernel(const float* __restrict__ up, const float* __restrict__ target, int HW, int mode, float wgt,
-                                                         float lc, float ls, float lo, const float* __restrict__ g_extra, float* __restrict__ sums,
-                                                         float* __restrict__ g_up) {
+                                                         float lc, float ls, float lo, float le, const float* __restrict__ g_extra,
+                                                         float* __restrict__ sums, float* __restrict__ g_up) {
     __shared__ float sh[8];
-    float s_c = 0.f, s_s = 0.f, s_o = 0.f;
+    float s_c = 0.f, s_s = 0.f, s_o = 0.f, s_e = 0.f;
     for (int i = blockIdx.x * 256 + threadIdx.x; i < HW; i += gridDim.x * 256) {
         const float t0 = __ldg(target + i), t1 = __ldg(target + HW + i), t2 = __ldg(target + 2 * (size_t)HW + i);
         const float tv[3] = {t0, t1, t2};
@@ -144,10 +170,19 @@ __global__ void __launch_bounds__(256) fusion_loss_kernel(const float* __restric
             s_s += huber_val(dm);
             gs += ls * huber_grad(dm) / HW;
         }
+        if constexpr (kEnt) {
+            float dh;
+            s_e += entropy_val_grad(sv, dh);
+            gs += le * dh / HW;
+        }
         g_up[3 * (size_t)HW + i] = gs;
     }
     const float a = block_sum_256(s_c, sh), b = block_sum_256(s_s, sh), c = block_sum_256(s_o, sh);
     if (threadIdx.x == 0) { atomicAdd(sums + 0, a); atomicAdd(sums + 1, b); atomicAdd(sums + 2, c); }
+    if constexpr (kEnt) {
+        const float e = block_sum_256(s_e, sh);
+        if (threadIdx.x == 0) atomicAdd(sums + 3, e);
+    }
 }
 
 // adjoint of upsample2x_render_kernel: g_img[p][c] = sum over the <= 16 destination pixels that read p of weight * g_up
@@ -199,8 +234,21 @@ int sfb_photometric_loss(const float* img, const float* sil, const float* rgb, c
     cudaStream_t st = as_stream(stream);
     SFB_CUDA(cudaMemsetAsync(sums, 0, 3 * sizeof(float), st));
     const int blocks = min(ceil_div(h * w, 256), sm_count() * 2);
-    photometric_loss_kernel<<<blocks, 256, 0, st>>>(img, sil, rgb, mask, h, w, scale, lambda_color, lambda_sil, lambda_opacity, sums, g_img, g_sil);
+    photometric_loss_kernel<false><<<blocks, 256, 0, st>>>(img, sil, rgb, mask, h, w, scale, lambda_color, lambda_sil, lambda_opacity, 0.f, sums, g_img,
+                                                           g_sil);
     return check_launch("photometric_loss");
+}
+
+int sfb_photometric_loss_ent(const float* img, const float* sil, const float* rgb, const float* mask, int h, int w, int scale, float lambda_color,
+                             float lambda_sil, float lambda_opacity, float lambda_entropy, float* sums, float* g_img, float* g_sil, void* stream) {
+    SFB_REQUIRE(img && sil && rgb && mask && sums && g_img && g_sil, "photometric_loss_ent: null pointer");
+    SFB_REQUIRE(h > 0 && w > 0 && scale >= 1, "photometric_loss_ent: bad sizes");
+    cudaStream_t st = as_stream(stream);
+    SFB_CUDA(cudaMemsetAsync(sums, 0, 4 * sizeof(float), st));
+    const int blocks = min(ceil_div(h * w, 256), sm_count() * 2);
+    photometric_loss_kernel<true><<<blocks, 256, 0, st>>>(img, sil, rgb, mask, h, w, scale, lambda_color, lambda_sil, lambda_opacity, lambda_entropy,
+                                                          sums, g_img, g_sil);
+    return check_launch("photometric_loss_ent");
 }
 
 int sfb_upsample2x_render(const float* img, const float* sil, int h, int w, float* up, void* stream) {
@@ -222,9 +270,25 @@ int sfb_fusion_loss_ex(const float* up, const float* target, int H, int W, int m
     cudaStream_t st = as_stream(stream);
     SFB_CUDA(cudaMemsetAsync(sums, 0, 3 * sizeof(float), st));
     const int blocks = min(ceil_div(H * W, 256), sm_count() * 2);
-    fusion_loss_kernel<<<blocks, 256, 0, st>>>(up, target, H * W, mode, weight, lambda_color, lambda_sil, lambda_opacity, g_extra, sums, g_up);
+    fusion_loss_kernel<false><<<blocks, 256, 0, st>>>(up, target, H * W, mode, weight, lambda_color, lambda_sil, lambda_opacity, 0.f, g_extra, sums,
+                                                      g_up);
     if (int rc = check_launch("fusion_loss(value)")) return rc;
     upsample2x_render_backward_kernel<<<ceil_div(h * w, 256), 256, 0, st>>>(g_up, h, w, g_img, g_sil);
     return check_launch("fusion_loss(adjoint)");
+}
+
+int sfb_fusion_loss_ent(const float* up, const float* target, int H, int W, int mode, float weight, float lambda_color, float lambda_sil,
+                        float lambda_opacity, float lambda_entropy, const float* g_extra, float* sums, float* g_up, int h, int w, float* g_img,
+                        float* g_sil, void* stream) {
+    SFB_REQUIRE(up && target && sums && g_up && g_img && g_sil, "fusion_loss_ent: null pointer");
+    SFB_REQUIRE(H == 2 * h && W == 2 * w && h > 0 && w > 0 && (mode == 0 || mode == 1), "fusion_loss_ent: the full-resolution planes must be 2x the render");
+    cudaStream_t st = as_stream(stream);
+    SFB_CUDA(cudaMemsetAsync(sums, 0, 4 * sizeof(float), st));
+    const int blocks = min(ceil_div(H * W, 256), sm_count() * 2);
+    fusion_loss_kernel<true><<<blocks, 256, 0, st>>>(up, target, H * W, mode, weight, lambda_color, lambda_sil, lambda_opacity, lambda_entropy, g_extra,
+                                                     sums, g_up);
+    if (int rc = check_launch("fusion_loss_ent(value)")) return rc;
+    upsample2x_render_backward_kernel<<<ceil_div(h * w, 256), 256, 0, st>>>(g_up, h, w, g_img, g_sil);
+    return check_launch("fusion_loss_ent(adjoint)");
 }
 }

@@ -72,6 +72,17 @@ def _check_sds_method(sds_method, where):
         raise ValueError(f'{where}: sds_method must be one of {SDS_METHODS} (got {sds_method!r})')
 
 
+def _check_lambda_entropy(lambda_entropy, where):
+    """ValueError, before any device work, for an entropy weight that is negative or not finite"""
+    le = float(lambda_entropy)
+    if not (math.isfinite(le) and le >= 0.0):
+        raise ValueError(f'{where}: lambda_entropy must be a finite value >= 0 (got {lambda_entropy!r})')
+
+
+# columns of the loss history (``Distiller.history``): the reference's loss_list, opacity_loss_list, entropy_loss_list and fusion_loss_list
+HISTORY_COLUMNS = ('volumetric', 'opacity', 'entropy', 'fusion')
+
+
 def normalize(x):  # utils/common_utils.py:9-13
     return torch.clip(x * 2 - 1.0, -1.0, 1.0)
 
@@ -105,7 +116,7 @@ def shard_views(views: list, rank: int, world_size: int) -> list:
 def view_seed(seed: int, itr: int, view: int, stream: int) -> int:
     """seed of the generator that serves ONE (iteration, view, stream) -- stream 0: photometric render, 1: fusion render, 2: PLMS noise, 3: evaluation
     render (``evaluate.evaluate_scene``, with iteration 0), 4: circle-path render (``evaluate.render_views`` for the fly-around gif, iteration 0), 5: VLDM
-    baseline samples (``baselines.sample_vldm_views``, iteration 0).
+    baseline samples (``baselines.sample_vldm_views``, iteration 0), 6: the periodic snapshot render of the photometric input view (``progress.py``).
     Keyed draws make a minibatch step independent of how its views are spread over ranks."""
     x = (seed * 0x9E3779B97F4A7C15 + itr * 0xBF58476D1CE4E5B9 + view * 0x94D049BB133111EB + stream * 0xD6E8FEB86659FD93) & 0xFFFFFFFFFFFFFFFF
     x ^= x >> 31
@@ -311,13 +322,15 @@ class Distiller:
     def __init__(self, ngp, vae, vldm, opt, cache: SceneCache, *, z_scale_factor=0.18215, plms_steps=50, start_fusion_step=1000,
                  lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3, seed=0, rank=0, world_size=1, process_group=None,
                  use_cuda_graph=True, fused_glue=True, percep=None, lambda_percep=0.1, start_percep_step=1000, views_per_step=None, max_batch=32,
-                 cond_scale=1.0, sds_method='plms'):
+                 cond_scale=1.0, sds_method='plms', lambda_entropy=0.0, max_itr=3000):
         _check_cond_scale(vldm, cond_scale, 'Distiller')
         _check_sds_method(sds_method, 'Distiller')
+        _check_lambda_entropy(lambda_entropy, 'Distiller')
         self.ngp, self.vae, self.vldm, self.opt, self.cache = ngp, vae, vldm, opt, cache
         self.z_scale_factor = z_scale_factor
         self.start_fusion_step = start_fusion_step
         self.lambda_color, self.lambda_sil, self.lambda_opacity = lambda_color, lambda_sil, lambda_opacity
+        self.lambda_entropy = float(lambda_entropy)    # entropy regulariser of both sub-steps (:236-241, :338-344); the reference's loop sets 0
         self.rank, self.world_size, self.pg = rank, world_size, process_group
         # None: the reference's two-update iteration on one view (one rank) / one view per rank (N ranks, legacy form); V: view-batched minibatch step
         self.views_per_step = views_per_step
@@ -342,6 +355,35 @@ class Distiller:
         self._keyed = False        # MultiSceneDistiller: the reference step draws from the keyed generators too (``_render_draws``)
         self.next_itr = 0          # the iteration after the last one run: what state_dict saves as ``itr``
         self.last = {}
+        # loss history (see ``history``): rows for max_itr iterations, grown by doubling should a step run past them
+        self._history = torch.full((max(int(max_itr), 1), len(HISTORY_COLUMNS)), math.nan, dtype=torch.float32, device=cache.input_rgb.device)
+
+    # ------------------------------------------------------------------------------------------------ loss history
+    @property
+    def history(self) -> torch.Tensor:
+        """[next_itr, 4] device tensor, row itr = the terms the reference logs at iteration itr (distillation.py:249-256, :349), columns
+        ``HISTORY_COLUMNS``: 'volumetric' (the photometric sub-step's loss, opacity and entropy included), 'opacity' (lambda_opacity *
+        opacity), 'entropy' (lambda_entropy * entropy) of the photometric sub-step, and 'fusion' (the fusion sub-step's SDS L1 plus the
+        perceptual term, or its EFT-bootstrap term; without opacity and entropy).  Each step writes its row with device-to-device copies, so
+        recording costs no host synchronisation.  nan marks a term not computed: the fusion term of a loop without diffusion, the photometric
+        terms of a rank that skipped the photometric sub-step in the view-batched step (the reference has no such case), and rows before the
+        iteration a run was resumed at from a checkpoint without history.  The view-batched step logs the mean over its V views (with
+        world_size R, over this rank's views' share of that mean)."""
+        return self._history[:self.next_itr]
+
+    def _history_rows(self, rows):
+        """grow the history buffer (nan rows, by doubling) until it holds ``rows`` rows"""
+        if rows > self._history.shape[0]:
+            grown = torch.full((max(2 * self._history.shape[0], rows), self._history.shape[1]), math.nan, dtype=self._history.dtype,
+                               device=self._history.device)
+            grown[:self._history.shape[0]].copy_(self._history)
+            self._history = grown
+
+    def _record(self, itr, col, values):
+        """row ``itr``, columns col.. of the history <- ``values`` (device tensor), without a host synchronisation"""
+        self._history_rows(itr + 1)
+        values = values.detach().reshape(-1)
+        self._history[itr, col:col + values.numel()].copy_(values)
 
     # ------------------------------------------------------------------------------------------------
     def _render_draws(self, rays_o, itr, view, stream, keyed):
@@ -372,12 +414,15 @@ class Distiller:
         return img.reshape(1, hw, hw, 3).permute(0, 3, 1, 2).contiguous(), ws.reshape(1, hw, hw, 1).permute(0, 3, 1, 2).contiguous()
 
     def _photometric_grad(self, idx, draws):
-        """photometric term of input view idx with the fused kernels: render, loss value and gradient (:216-234), backward; returns the loss"""
+        """photometric term of input view idx with the fused kernels: render, loss value and gradient (:216-241), backward; returns the loss
+        and leaves its [4] logged terms (``image_glue.photometric_loss``) in ``last['photo_terms']``"""
         c = self.cache
         img, ws, hw = self._render(c.input_rays_o[idx], c.input_rays_d[idx], draws)
-        loss, g_img, g_ws = glue.photometric_loss(img.detach(), ws.detach(), c.input_rgb[idx], c.input_mask[idx], hw, hw, int(self.opt.hw_scale),
-                                                  self.lambda_color, self.lambda_sil, self.lambda_opacity)
+        loss, g_img, g_ws, terms = glue.photometric_loss(img.detach(), ws.detach(), c.input_rgb[idx], c.input_mask[idx], hw, hw,
+                                                         int(self.opt.hw_scale), self.lambda_color, self.lambda_sil, self.lambda_opacity,
+                                                         lambda_entropy=self.lambda_entropy, return_terms=True)
         torch.autograd.backward((img, ws), (g_img, g_ws))
+        self.last['photo_terms'] = terms
         return loss
 
     def photometric_substep(self, itr: int):
@@ -389,9 +434,11 @@ class Distiller:
         if self.opt.cuda_ray and itr % 16 == 0:                                               # :181-182
             self.ngp.update_extra_state()
         draws = self._render_draws(c.input_rays_o[idx], itr, 0, 0, self._keyed)              # keyed: view 0, whichever input view is drawn
+        self.last['input_view'] = idx
         if self.fused_glue:
             self.optimizer.zero_grad()                                                        # :244
             loss = self._photometric_grad(idx, draws)
+            terms = self.last['photo_terms']
         else:
             image, sil = self._render_nchw(c.input_rays_o[idx], c.input_rays_d[idx], draws)
             scale = 1.0 / self.opt.hw_scale
@@ -402,12 +449,19 @@ class Distiller:
             loss = self.lambda_color * color_err + self.lambda_sil * sil_err                  # :227
             opacity = torch.sqrt(sil ** 2 + .01).mean()                                       # :233
             loss = loss + self.lambda_opacity * opacity                                       # :234
+            entropy = torch.zeros_like(loss)
+            if self.lambda_entropy > 0:
+                alphas = sil.clamp(1e-5, 1 - 1e-5)                                            # :238-240
+                entropy = (- alphas * torch.log2(alphas) - (1 - alphas) * torch.log2(1 - alphas)).mean()
+                loss = loss + self.lambda_entropy * entropy                                   # :241
             self.optimizer.zero_grad()                                                        # :244
             loss.backward()
             loss = loss.detach()
+            terms = torch.stack((loss, (self.lambda_opacity * opacity).detach(), (self.lambda_entropy * entropy).detach()))   # :254-256
         # replicated sub-step: for N>1 the reduce only removes atomic-order drift so that ranks stay bit-identical
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))
         self.optimizer.scheduler_step()                                                       # :247
+        self._record(itr, 0, terms[:3])                                                       # :254-256
         self.last['photo_loss'] = loss
         self.next_itr = itr + 1
         return loss
@@ -442,7 +496,12 @@ class Distiller:
             fusion_loss = self.lambda_color * huber(image, noisy_rgb).abs().mean() + self.lambda_sil * huber(sil, noisy_mask).abs().mean()
         opacity = torch.sqrt(sil ** 2 + .01).mean()                                           # :336
         loss = fusion_loss + self.lambda_opacity * opacity                                    # :344
+        if self.lambda_entropy > 0:
+            alphas = sil.clamp(1e-5, 1 - 1e-5)                                                # :340-342
+            entropy = (- alphas * torch.log2(alphas) - (1 - alphas) * torch.log2(1 - alphas)).mean()
+            loss = loss + self.lambda_entropy * entropy                                       # :344
         loss.backward()                                                                       # :345
+        self._record(itr, 3, fusion_loss)                                                     # :349
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))   # :352
         self.last['fusion_loss'] = loss.detach()
         return loss.detach()
@@ -451,7 +510,8 @@ class Distiller:
         """the same sub-step on target view vi (conditioning ``feats``) with the fused image-space kernels, then Adam (:352)"""
         if itr > self.start_fusion_step and max_thres is None:
             max_thres = u.clamp(min=0.0, max=0.99).item()                                     # :303
-        loss = self._fusion_views(itr, [vi], feats, max_thres, self._keyed, 1.0)[0]
+        loss, logged = self._fusion_views(itr, [vi], feats, max_thres, self._keyed, 1.0)[0]
+        self._record(itr, 3, logged)                                                          # :349
         self.optimizer.step(grad_scale=self.optimizer.sync_grads(self.world_size, self.pg))   # :352
         self.last['fusion_loss'] = loss
         return loss
@@ -461,7 +521,7 @@ class Distiller:
         (bilinear x2 to NCHW for the VAE, loss value + gradient at full resolution, adjoint of the bilinear back to the render's [N,3] / [N]
         outputs): renders, ONE SDS target batch passed through ``pred_img_hook`` (or the EFT bootstrap), each view's gradient scaled by
         ``scale``.  PLMS draws: keyed per view (``plms_noise`` or ``KeyedNoise``) when ``keyed``, else the sampler's own.  Returns the views'
-        losses, unscaled; the caller steps the optimiser."""
+        (loss, logged fusion term) pairs (``_fusion_grad``), unscaled; the caller steps the optimiser."""
         renders = self._fusion_renders(itr, views, keyed)
         pred = [None] * len(views)
         if itr > self.start_fusion_step:                                                      # :294
@@ -546,24 +606,28 @@ class Distiller:
 
     def _fusion_grad(self, itr, img, ws, hw, up, vi, pred_img, max_thres, scale=1.0):
         """loss value and gradient of target view vi (:307-344; SDS against ``pred_img`` [3,2hw,2hw], or the EFT bootstrap when it is None),
-        backward (:345) of the gradient times ``scale``; returns the loss.  The caller steps the optimiser (:352)."""
+        backward (:345) of the gradient times ``scale``; returns the loss and the fusion term the reference logs (:349: the SDS L1 plus the
+        perceptual term, or the EFT-bootstrap term; no opacity or entropy).  The caller steps the optimiser (:352)."""
         if pred_img is not None:
             weight = 1.0 - plms_sigmoid(plms_log_snr(float(max_thres)))                      # 1 - alpha_cumprod of the run's first noise level (:307)
             g_extra, percep_term = None, None
             if self.percep is not None and itr >= self.start_percep_step:                     # :176-178, :312-314: value and gradient together
                 pv, pg = self.percep.value_and_grad(up[:3], pred_img, normalize=True)
                 percep_term, g_extra = pv * self.lambda_percep, pg * self.lambda_percep
-            loss, g_img, g_ws = glue.fusion_loss(up, pred_img, hw, hw, 'sds', weight, self.lambda_color, self.lambda_sil, self.lambda_opacity,
-                                                 g_extra=g_extra)
+            loss, g_img, g_ws, terms = glue.fusion_loss(up, pred_img, hw, hw, 'sds', weight, self.lambda_color, self.lambda_sil,
+                                                        self.lambda_opacity, g_extra=g_extra, lambda_entropy=self.lambda_entropy, return_terms=True)
+            logged = terms[3]
             if percep_term is not None:
                 loss = loss + percep_term
+                logged = logged + percep_term
         else:                                                                                 # EFT bootstrap :316-329
-            loss, g_img, g_ws = glue.fusion_loss(up, self.cache.target_eft_image[vi], hw, hw, 'eft', 1.0, self.lambda_color, self.lambda_sil,
-                                                 self.lambda_opacity)
+            loss, g_img, g_ws, terms = glue.fusion_loss(up, self.cache.target_eft_image[vi], hw, hw, 'eft', 1.0, self.lambda_color,
+                                                        self.lambda_sil, self.lambda_opacity, lambda_entropy=self.lambda_entropy, return_terms=True)
+            logged = terms[3]
         if scale != 1.0:
             g_img, g_ws = g_img * scale, g_ws * scale
         torch.autograd.backward((img, ws), (g_img, g_ws))                                     # :345
-        return loss
+        return loss, logged
 
     def step(self, itr: int, max_thres: Optional[float] = None):
         """one iteration of the reference's main loop (distillation.py:174-352); returns the two losses as device scalars"""
@@ -591,12 +655,16 @@ class Distiller:
         mine = shard_views(views, r, R)
         self.ngp.train()
         self.optimizer.zero_grad()
-        loss_a = loss_b = torch.zeros((), device=c.input_rgb.device)
+        loss_a = loss_b = logged_b = torch.zeros((), device=c.input_rgb.device)
         if self.opt.cuda_ray and itr % 16 == 0:
             self.ngp.update_extra_state()
+        self.last['input_view'] = idx
         # ---- photometric term: one rank (round-robin over iterations), gradient joins the step's single all-reduce
         if itr % R == r:
             loss_a = self._photometric_grad(idx, self._render_draws(c.input_rays_o[idx], itr, idx, 0, True))
+            self._record(itr, 0, self.last['photo_terms'][:3])
+        else:
+            self._record(itr, 0, torch.full((3,), math.nan, device=c.input_rgb.device))
         # ---- fusion term over this rank's views, in batches of at most max_batch, gradient = mean over the step's V views
         sds = itr > self.start_fusion_step
         if sds and max_thres is None:
@@ -607,8 +675,10 @@ class Distiller:
         for lo in range(0, len(mine), self.max_batch):
             chunk = mine[lo:lo + self.max_batch]
             feats = c.target_features[chunk] if sds else None         # cache fields take int, one-row slice or list indices (bench.py's staged cache)
-            for lv in self._fusion_views(itr, chunk, feats, max_thres, True, inv_v, first=lo == 0):
+            for lv, gv in self._fusion_views(itr, chunk, feats, max_thres, True, inv_v, first=lo == 0):
                 loss_b = loss_b + lv * inv_v
+                logged_b = logged_b + gv * inv_v
+        self._record(itr, 3, logged_b if mine else torch.full((1,), math.nan, device=c.input_rgb.device))
         self.optimizer.sync_grads(R, self.pg)              # the step's ONE collective: sum of every rank's (photometric + fusion) gradient
         self.optimizer.step(grad_scale=1.0)
         self.optimizer.scheduler_step()                                                        # :247
@@ -625,7 +695,9 @@ class Distiller:
                     sds_method=self.sds_method, use_diffusion=bool(use_diffusion), lambda_color=self.lambda_color, lambda_sil=self.lambda_sil,
                     lambda_opacity=self.lambda_opacity, lambda_percep=self.lambda_percep, start_fusion_step=self.start_fusion_step,
                     start_percep_step=self.start_percep_step, plms_steps=self.sampler.plms_steps, fused_glue=self.fused_glue,
-                    percep=self.percep is not None, z_scale_factor=self.z_scale_factor, keyed=self._keyed)
+                    percep=self.percep is not None, z_scale_factor=self.z_scale_factor, keyed=self._keyed,
+                    # only when on: checkpoints made before the entropy term existed carry no such key and continue at lambda_entropy 0
+                    **({'lambda_entropy': self.lambda_entropy} if self.lambda_entropy != 0 else {}))
 
     def _scene_state(self, itr, use_diffusion):
         """this scene's part of a checkpoint: everything but the global generators"""
@@ -633,7 +705,8 @@ class Distiller:
         return dict(version=CHECKPOINT_VERSION, itr=int(itr), world_size=self.world_size, seed=self.seed,
                     fingerprint=self.fingerprint(use_diffusion), cache=cache_digest(self.cache),
                     ngp={k: v.detach().to('cpu', copy=True) for k, v in self.ngp.state_dict().items()}, ngp_extra=extra,
-                    optimizer=self.optimizer.state_dict(), gen=self.gen.get_state())
+                    optimizer=self.optimizer.state_dict(), gen=self.gen.get_state(),
+                    history=self._history[:int(itr)].to('cpu', copy=True))
 
     def state_dict(self, itr: Optional[int] = None, use_diffusion=True) -> dict:
         """everything needed to continue this run at iteration ``itr`` (default: the one after the last step run): a format version,
@@ -680,6 +753,9 @@ class Distiller:
             if tuple(sd['ngp'][k].shape) != tuple(v.shape):
                 raise _mismatch(f'ngp.{k} shape', tuple(sd['ngp'][k].shape), tuple(v.shape))
         self.optimizer.check_state(sd['optimizer'])
+        hist = sd.get('history')            # optional: checkpoints made before the loss history have none
+        if hist is not None and (hist.dim() != 2 or hist.shape[1] != len(HISTORY_COLUMNS) or hist.shape[0] > sd['itr']):
+            raise _mismatch('history shape', tuple(hist.shape), f'(<= {sd["itr"]}, {len(HISTORY_COLUMNS)})')
 
     def _load_scene_state(self, sd):
         self.ngp.load_state_dict(sd['ngp'])          # copies into the existing tensors: the parameters stay views of the flat buffer
@@ -688,6 +764,11 @@ class Distiller:
         self.optimizer.load_state_dict(sd['optimizer'])
         self.gen.set_state(sd['gen'])
         self.next_itr = int(sd['itr'])
+        self._history.fill_(math.nan)
+        hist = sd.get('history')
+        if hist is not None:
+            self._history_rows(hist.shape[0])
+            self._history[:hist.shape[0]].copy_(hist)
 
     def load_state_dict(self, sd, use_diffusion=True):
         """continue from ``state_dict``'s ``sd``: ``check_state`` first (ValueError before any device state is touched), then the network,
@@ -726,7 +807,8 @@ class MultiSceneDistiller:
     ``plms_noise(scene) -> noise_fn``, the per-scene counterparts of ``Distiller.render_noise`` and ``PLMSSampler.noise_fn``.
 
     Not supported: ``views_per_step`` (NotImplementedError), ``fused_glue=False`` and ``opt.hw_scale != 2`` (NotImplementedError), scenes of
-    different image, latent or ray sizes (ValueError), CPU tensors (RuntimeError)."""
+    different image, latent or ray sizes (ValueError), CPU tensors (RuntimeError).  ``lambda_entropy`` and ``max_itr`` (the rows of each
+    scene's loss history) pass to every scene's ``Distiller``."""
 
     def __init__(self, ngps, vae, vldm, opt, caches, *, seeds, percep=None, max_batch=8, cond_scale=1.0, sds_method='plms', **kw):
         _check_cond_scale(vldm, cond_scale, 'MultiSceneDistiller')
@@ -767,6 +849,11 @@ class MultiSceneDistiller:
 
     def __len__(self):
         return len(self.scenes)
+
+    @property
+    def history(self) -> list:
+        """every scene's loss history (``Distiller.history``), in scene order"""
+        return [d.history for d in self.scenes]
 
     @property
     def render_noise(self):
@@ -832,7 +919,9 @@ class MultiSceneDistiller:
                     self.scenes[k].last['unet_calls'] = calls[k]
             for j, k in enumerate(ks):
                 d = self.scenes[k]
-                losses[k] = d.last['fusion_loss'] = d._fusion_grad(itr, *renders[j], views[j], pred[j], mts[j])
+                losses[k], logged = d._fusion_grad(itr, *renders[j], views[j], pred[j], mts[j])
+                d.last['fusion_loss'] = losses[k]
+                d._record(itr, 3, logged)                                                      # :349
                 d.optimizer.step()                                                             # :352 (one rank: grad_scale 1)
             del renders
         if sds:
@@ -1043,7 +1132,7 @@ class NativeSceneBuilder:
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
                       process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                      cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False):
+                      cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -1065,8 +1154,18 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     that shading under a headlight (``evaluate.render_views``), at ambient ratio 0.1 for the lit shadings ('lambertian', 'textureless') so the
     geometry shows, 1.0 for 'normal' and 'albedo'.
 
-    Not reproduced: the matplotlib loss plots and the periodic ``_vis.jpg`` renders (:355-388) -- logging, outside the hot path;
-    ``on_iteration(itr, distiller)`` is the hook for them (``distiller.ngp.render_batched`` is the same call the reference makes).
+    ``lambda_entropy`` weights the reference's entropy regulariser of both sub-steps (:236-241, :338-344; its loop sets 0, the default
+    here); a negative value is a ValueError.  Every step records the logged terms in ``Distiller.history`` on the device.
+
+    ``progress_every=K`` writes the reference's periodic outputs (:355-388; ``progress.ProgressWriter``) after every iteration ``itr`` with
+    ``itr % K == 0`` (the reference: K = 20): ``{args.exp_dir}/log/{seq_name}_loss.jpg`` and ``{seq_name}_fusionloss.jpg``, the loss curves
+    of every iteration so far drawn with Pillow, and ``{seq_name}_vis.jpg``, the eval-mode render | silhouette of the iteration's photometric
+    input view through the builder's ``eval_views`` rays (a builder without ``eval_views`` fails before the loop).  Writing them draws from
+    no global generator and leaves the network in train mode, so the run's steps are those of a run without them.  With a process group
+    rank 0 writes.  None (the default) writes nothing; K <= 0 is a ValueError.  The tqdm bar and the ``running_loss`` print stay out.
+    With a process group the plots show rank 0's own history (``Distiller.history``): in the view-batched step its photometric terms exist
+    every R-th iteration only, so those curves are dots rather than lines, and its fusion curve is its views' share of the step's mean,
+    not the mean over all V views.
     ``scene_valid_region`` is accepted and unused, as in the reference's loop body (:192-195 overwrites the region with ones), and so is
     ``loss_fn_vgg`` unless ``evaluate``.  Extensions, keyword-only: ``views_per_step`` (view-batched step, see the module docstring; with
     torch.distributed initialised and ``process_group`` given the views are sharded over its ranks), ``seed``, ``evaluate``, ``visualize``,
@@ -1099,6 +1198,7 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distillation_loop')
+    _check_lambda_entropy(lambda_entropy, 'distillation_loop')
     if use_diffusion:
         _check_cond_scale(vldm, cond_scale, 'distillation_loop')
     rank, world = 0, 1
@@ -1108,17 +1208,19 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     def make(ngps, caches, percep, seed):
         return Distiller(ngps[0], vae, vldm, opt, caches[0], plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0,   # :148-160
                          lambda_opacity=1e-3, seed=seed, rank=rank, world_size=world, process_group=process_group, percep=percep, lambda_percep=0.1,
-                         start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
+                         start_percep_step=1000, views_per_step=views_per_step, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method,
+                         lambda_entropy=lambda_entropy, max_itr=max_itr)
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
-                                     visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale), checkpoint_every, resume)
+                                     visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale), checkpoint_every, resume,
+                                     progress_every)
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
                    evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                   cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False):
+                   cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -1134,20 +1236,23 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     SDS target, 'plms' or 'onestep', as ``distillation_loop(sds_method=...)``; a chunk's one-step targets are one ``forward_noloss`` call.
     ``checkpoint_every`` / ``resume``: as ``distillation_loop``'s, one ``{save_dir}/checkpoints/{seq_name}.ckpt`` per scene (scene k's part
     of ``MultiSceneDistiller.state_dict``).  Resuming needs a checkpoint at the same iteration for every scene of the call, or none (then
-    the call starts fresh); anything else is a ValueError naming the scenes.
+    the call starts fresh); anything else is a ValueError naming the scenes.  ``lambda_entropy`` / ``progress_every``: as
+    ``distillation_loop``'s, every scene's entropy weight, history and progress files, scene k's snapshot jitter keyed by ``seed + k``.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distill_scenes')
+    _check_lambda_entropy(lambda_entropy, 'distill_scenes')
     if use_diffusion:
         _check_cond_scale(vldm, cond_scale, 'distill_scenes')
 
     def make(ngps, caches, percep, base):
         return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
-                                   lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method)
+                                   lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method,
+                                   lambda_entropy=lambda_entropy, max_itr=max_itr)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
                              loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale),
-                             checkpoint_every, resume)
+                             checkpoint_every, resume, progress_every)
 
 
 def _baselines(enabled, vae, vldm, cond_scale):
@@ -1265,14 +1370,17 @@ def _write_checkpoints(dist, paths, itr, use_diffusion, base_seed):
 
 
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
-                      loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None, checkpoint_every=None, resume=False):
+                      loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None, checkpoint_every=None, resume=False,
+                      progress_every=None):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
     ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
     ``max_itr`` iterations and one saved network per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
     grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``); with ``baselines`` (``_baselines``), the EFT and VLDM
-    scores, metrics files and gifs after it; with ``checkpoint_every`` / ``resume`` the checkpoints of ``distillation_loop``'s docstring.
-    Returns the networks."""
+    scores, metrics files and gifs after it; with ``checkpoint_every`` / ``resume`` the checkpoints and with ``progress_every`` the progress
+    files of ``distillation_loop``'s docstring.  Returns the networks."""
     from .lpips_vgg import PerceptualLoss
+    from .progress import ProgressWriter, check_progress_every
+    check_progress_every(progress_every)
     if checkpoint_every is not None and (isinstance(checkpoint_every, bool) or not isinstance(checkpoint_every, int) or checkpoint_every < 1):
         raise ValueError(f'checkpoint_every must be a positive int or None (got {checkpoint_every!r})')
     ckpt_paths = _checkpoint_paths(save_dir, scenes)
@@ -1281,7 +1389,7 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     visualize_shadings = tuple(visualize_shadings)
     if not all(isinstance(sh, str) and sh and '/' not in sh for sh in visualize_shadings):
         raise ValueError(f'visualize_shadings must be shading names, got {visualize_shadings!r}')
-    if visualize:
+    if visualize or progress_every is not None:
         from .video import require_pillow
         require_pillow()
     if baselines is not None:
@@ -1289,9 +1397,11 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
         check_baseline_options(baselines['vldm'], baselines['cond_scale'], use_diffusion)
         from .video import require_pillow
         require_pillow()
-    for flag, name, sig in ((evaluate or visualize or baselines is not None, 'eval_views', '(scene_cameras, scene_rgb, scene_mask)'), (visualize, 'circle_views', '(scene_cameras)')):
+    scored = evaluate or visualize or baselines is not None
+    need_views = scored or progress_every is not None
+    for flag, name, sig in ((need_views, 'eval_views', '(scene_cameras, scene_rgb, scene_mask)'), (visualize, 'circle_views', '(scene_cameras)')):
         if flag and not callable(getattr(builder, name, None)):
-            raise TypeError(f'{_needs(name, evaluate, visualize)} needs the scene builder to provide '
+            raise TypeError(f'{_needs(name, evaluate, visualize, baselines is not None)} needs the scene builder to provide '
                             f'{name}{sig}; {type(builder).__name__} has none')
     exp_dir = getattr(args, 'exp_dir', save_dir)
     for sc in scenes:
@@ -1299,7 +1409,11 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     os.makedirs(f'{exp_dir}/render_gifs/', exist_ok=True)
     os.makedirs(save_dir, exist_ok=True)
     device = torch.device('cuda', gpu) if isinstance(gpu, int) else torch.device(gpu)
-    eval_views = [builder.eval_views(cams, rgb, mask).to(device) for _, cams, rgb, mask, _, _ in scenes] if evaluate or visualize or baselines else None
+    all_views = [builder.eval_views(cams, rgb, mask) for _, cams, rgb, mask, _, _ in scenes] if need_views else None
+    eval_views = [v.to(device) for v in all_views] if scored else None
+    # the snapshots render input views only: a copy of those rows, so the other views' rays need not stay on the device for the run
+    input_views = [_view_rows(v, sc[5]).to(device) for v, sc in zip(all_views, scenes)] if progress_every is not None else None
+    del all_views
     circles = [tuple(t.to(device) for t in builder.circle_views(cams)) for _, cams, _, _, _, _ in scenes] if visualize else None
     caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
               for _, cams, rgb, mask, _, input_idx in scenes]
@@ -1324,6 +1438,9 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
         else:
             base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
         dist = make(ngps, caches, perceptual_loss, base_seed)
+        progress = None
+        if progress_every is not None and getattr(dist, 'rank', 0) == 0:
+            progress = ProgressWriter(exp_dir, [sc[0] for sc in scenes], input_views, [sc[5] for sc in scenes], opt)
         start = 0
         if saved is not None:                  # restores the global generators too: nothing may draw between here and the first step
             multi = isinstance(dist, MultiSceneDistiller)
@@ -1336,6 +1453,8 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
                 dist.photometric_substep(itr)
             if checkpoint_every is not None and ((itr + 1) % checkpoint_every == 0 or itr == max_itr - 1):
                 _write_checkpoints(dist, ckpt_paths, itr + 1, use_diffusion, base_seed)
+            if progress is not None and itr % progress_every == 0:                                                   # :355
+                progress.write(itr, getattr(dist, 'scenes', [dist]))
             if on_iteration is not None:
                 on_iteration(itr, dist)
         torch.cuda.synchronize(device)
@@ -1364,8 +1483,16 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     return ngps
 
 
-def _needs(name, evaluate, visualize):
+def _view_rows(views, idx):
+    """the rows ``idx`` of ``views`` (``evaluate.EvalViews``) as new tensors"""
+    from .evaluate import EvalViews
+    idx = [int(i) for i in idx]
+    return EvalViews(*[getattr(views, f)[idx] for f in EvalViews.__dataclass_fields__])
+
+
+def _needs(name, evaluate, visualize, baselines=False):
     """the option that asked the scene builder for ``name``, for the error message"""
     if name == 'eval_views':
-        return 'evaluate=True' if evaluate else 'visualize=True' if visualize else 'evaluate_baselines=True'
+        return ('evaluate=True' if evaluate else 'visualize=True' if visualize else 'evaluate_baselines=True' if baselines
+                else 'progress_every')
     return 'visualize=True'

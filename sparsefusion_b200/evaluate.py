@@ -72,11 +72,12 @@ def image_metrics(pred: torch.Tensor, gt: torch.Tensor):
 
 @torch.no_grad()
 def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, seed: int, stream: int, shading: str = 'albedo',
-                 ambient_ratio: float = 1.0):
+                 ambient_ratio: float = 1.0, itr: int = 0, view_ids=None):
     """(images [V, H, W, 3] fp32, silhouettes [V, H, W]) of V views (rays [V, H*W, 3], ``hw`` = (H, W)) with the reference's eval-mode render
     call (distillation.py:404-406, :480-482).  Its ``perturb=True`` jitter, which the reference draws from torch's unseeded global generator,
-    comes from the CUDA generator seeded with ``view_seed(seed, 0, view, stream)`` inside ``torch.random.fork_rng``, so the renders are
-    reproducible and the callers' generators are left as they were.  ``ngp.training`` is restored on return.  A shading other than 'albedo'
+    comes from the CUDA generator seeded with ``view_seed(seed, itr, view, stream)`` inside ``torch.random.fork_rng``, so the renders are
+    reproducible and the callers' generators are left as they were; ``view`` is the view's index in ``rays_o``, or its entry of
+    ``view_ids``.  ``ngp.training`` is restored on return.  A shading other than 'albedo'
     (NeRFNetwork.forward's) is lit by a headlight, light_d = safe_normalize(rays_o[v][0]), so a turntable of views does not flicker."""
     dev = rays_o.device
     if dev.type != 'cuda':
@@ -92,7 +93,7 @@ def render_views(ngp, rays_o: torch.Tensor, rays_d: torch.Tensor, hw, opt, *, se
         with torch.cuda.device(dev):
             for v in range(V):
                 with torch.random.fork_rng(devices=[dev]):
-                    torch.cuda.manual_seed(view_seed(seed, 0, v, stream))
+                    torch.cuda.manual_seed(view_seed(seed, itr, v if view_ids is None else int(view_ids[v]), stream))
                     light = {} if shading == 'albedo' else {'light_d': torch.nn.functional.normalize(rays_o[v][0], dim=0, eps=1e-10)}
                     out = ngp.render_batched(rays_o[v][None], rays_d[v][None], batched=True, perturb=True, bg_color=0, ambient_ratio=ambient_ratio,
                                              shading=shading, force_all_rays=True, **light, **vars(opt))
