@@ -14,6 +14,8 @@ with gamma, ``violations`` and ``assert_within`` from ``field_fp64`` (Higham's m
 
 ``emulate`` evaluates the kernel's arithmetic in the kernel's k order (fp64 products of the tf32 operand words, fp32 partial sums),
 with switches that inject single defects; the host tests use it to show which defects the bound sees.
+
+``entry`` turns an oracle/insitu record of ``ops.conv2d_nhwc`` into the geometry and memory layout tests/test_conv_fp64_gpu.py replays.
 """
 from __future__ import annotations
 
@@ -297,3 +299,42 @@ def max_ratio(got: torch.Tensor, bnd: torch.Tensor, ref: torch.Tensor) -> float:
     r = err / (bnd + ATOL)
     r = torch.where(torch.isnan(r), torch.full_like(r, math.inf), r)
     return float(r.max()) if r.numel() else 0.0
+
+
+# ------------------------------------------------------------------------------------------------ recorded launches
+def nhwc_meta(t: torch.Tensor):
+    """(NB, H, W, C, ld, off) of an NHWC tensor or channel slice of one: ld its row stride, off its first channel within a row (0 when
+    the slice does not sit inside one row)"""
+    nb, h, w, c = t.shape
+    ld = t.stride(2)
+    off = t.storage_offset() % ld
+    return nb, h, w, c, ld, (off if off + c <= ld else 0)
+
+
+def rows_meta(t: torch.Tensor):
+    """(rows, C, ld, off) of a row-major [..., C] tensor with a uniform row stride ld, off as in ``nhwc_meta``"""
+    c = t.shape[-1]
+    ld = t.stride(-2) if t.dim() >= 2 else c
+    off = t.storage_offset() % ld if ld else 0
+    return t.numel() // c, c, ld, (off if off + c <= ld else 0)
+
+
+def same_ptr(a: Optional[torch.Tensor], b: Optional[torch.Tensor]) -> bool:
+    return a is not None and b is not None and a.data_ptr() == b.data_ptr()
+
+
+def entry(r) -> Optional[Dict]:
+    """the replay entry of an oracle/insitu record of ``ops.conv2d_nhwc`` (None for any other launch): geometry, row strides and slice
+    offsets of x, out and the residual, the switches, and ``alias`` where two of them start at the same address"""
+    if r.op != 'conv2d_nhwc':
+        return None
+    t, s = r.orig, r.s
+    x, y, res = t['x'], t['out'], t['residual']
+    nb, h, w, cin, ldx, xoff = nhwc_meta(x)
+    ldo, ooff = nhwc_meta(y)[4:]
+    ldr, roff = nhwc_meta(res)[4:] if res is not None else (0, 0)
+    alias = [n for a, b, n in ((x, y, 'x=out'), (res, y, 'res=out'), (x, res, 'x=res')) if same_ptr(a, b)]
+    return dict(NB=nb, H=h, W=w, Cin=cin, ldx=ldx, xoff=xoff, Cout=s['cout'], KH=s['kh'], KW=s['kw'], stride=s['stride'], pad=s['pad'],
+                pad_after=s['pad_after'], ldo=ldo, ooff=ooff, bias=t['bias'] is not None, residual=res is not None, ldr=ldr, roff=roff,
+                accumulate=s['accumulate'], w_split=t['w_split'] is not None, dyn=s['dyn'], splits=s['splits'], bn=s['bn'],
+                alias=','.join(alias), family=r.family, label=r.label)

@@ -7,11 +7,14 @@ The per-launch tests (tests/test_conv_fp64_gpu.py, tests/test_simt_fp64_gpu.py) 
 so they cannot see an operand read before its producer finished: programmatic dependent launch (PDL), CUDA-graph replays whose
 intermediates sit at the same address every time, the UNet's side stream, the split-K arena.  Here the operands are the model's own.
 
-``Recorder`` wraps the ``ops.*`` front ends (the list of the two recorders above) and ``_lib.call``.  Each front-end launch becomes a ``Rec``:
-the op, its scalars, references to its input and output tensors (views, slices and strides as passed), the stream it was issued on,
-whether it was captured into a graph, the library kernels it launched (``sfb_launch_count``) and their traced names.  Every tensor stays
-alive as long as the recorder, so the caching allocator reuses no buffer inside a recorded evaluation: write-after-read hazards between
-launches are out of scope.
+``Recorder`` is the one wrapper of the ``ops.*`` front ends and ``_lib.call``.  Each front-end launch becomes a ``Rec``: the op, its
+scalars, references to its input and output tensors (views, slices and strides as passed), the stream it was issued on, whether it was
+captured into a graph, the library kernels it launched (``sfb_launch_count``) and their traced names.  Every tensor stays alive as long as
+the recorder, so the caching allocator reuses no buffer inside a recorded evaluation: write-after-read hazards between launches are out of
+scope.  Each C ABI call made outside a front end becomes a ``Call``: its arguments bound to the header's parameter names.
+
+``Catalogue`` turns the records of oracle/model_runs' evaluations into the entries the per-launch replay tests replay, through the
+``entry`` function of oracle/conv_fp64.py, oracle/simt_fp64.py or oracle/step_fp64.py.
 
 A launch that writes memory an earlier record (or the launch itself: x=out, res=out, accumulate into a pre-filled ``out``) read or wrote
 would leave that record without the values it saw.  Right before such a launch the recorder clones the overlapping tensor and the record
@@ -27,8 +30,10 @@ weight stages unless ``dynamic_weights``) against the storages of the prepared p
 from __future__ import annotations
 
 import ctypes
+import gc
 import inspect
 import math
+import re
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional
 
@@ -62,6 +67,18 @@ class Rec:
     def __post_init__(self):
         if not self.orig:
             self.orig = dict(self.t)
+
+
+@dataclass
+class Call:
+    op: str                 # the C ABI symbol
+    args: Dict              # parameter name (the last identifier of its declaration in the header) -> argument
+    family: str = ''
+    at: int = 0             # front-end records made before the call
+
+
+# pointer arguments the recorder copies at call time, with their float counts: the per-row scalar tables of the sampler updates
+BY_VALUE = {'row_scalars': lambda a: 5 * a['rows']}
 
 
 @dataclass
@@ -113,7 +130,20 @@ def storage_of(t: torch.Tensor) -> int:
     return t.untyped_storage().data_ptr()
 
 
+def device_floats(ptr: int, n: int) -> torch.Tensor:
+    """a copy of n floats at a device address, in stream order"""
+    class _View:
+        __cuda_array_interface__ = dict(shape=(n,), typestr='<f4', data=(ptr, False), version=3)
+    return torch.as_tensor(_View(), device='cuda').clone()
+
+
 # ------------------------------------------------------------------------------------------------ recorder
+def c_params() -> Dict[str, List[str]]:
+    """symbol -> parameter names of the C ABI header: the last identifier of each declaration"""
+    from sparsefusion_b200 import _lib as lib
+    return {n: [re.search(r'(\w+)\s*$', d).group(1) for d in decls] for n, (_, decls) in lib.parse_header().items()}
+
+
 def _specs():
     """op -> (inputs, outputs given before the launch, outputs after the launch, scalars) as functions of the bound arguments"""
     def conv(a, y):
@@ -139,7 +169,7 @@ def _specs():
         softmax_rows=(lambda a, y: (dict(x=a['x']), dict(out=y), dict(scale=float(a['scale']))), lambda a: a['out']),
         upsample2x=(lambda a, y: (dict(x=a['x']), dict(out=y), {}), lambda a: None),
         nchw_to_nhwc=(lambda a, y: (dict(src=a['src']), dict(out=a['dst'][..., a['c_off']:a['c_off'] + a['src'].shape[1]]),
-                                    dict(round=bool(a['round_to_tf32']))),
+                                    dict(round=bool(a['round_to_tf32']), c_off=a['c_off'])),
                       lambda a: a['dst'][..., a['c_off']:a['c_off'] + a['src'].shape[1]]),
         nhwc_to_nchw=(lambda a, y: (dict(src=a['src']), dict(out=y), {}), lambda a: None),
         im2col4=(lambda a, y: (dict(x=a['x']), dict(out=y), dict(kh=a['kh'], kw=a['kw'], pad=a['pad'])), lambda a: None),
@@ -153,10 +183,11 @@ PLMS_CALLS = ('sfb_plms_update_rows', 'sfb_plms_update_rows_cfg')
 
 
 class Recorder:
-    """``with Recorder() as r: <model evaluation>`` -> ``r.recs`` (front-end launches in issue order) and ``r.unchecked`` (C ABI launches
-    that bypass the front ends: (name, kernels, traced names)).  ``family`` labels the records; ``captured_only`` passes launches outside a
-    graph capture straight through (UnetGraph's eager warm-up).  ``unattributed`` collects traced kernel names that no record or listed
-    launch accounts for.
+    """``with Recorder() as r: <model evaluation>`` -> ``r.recs`` (front-end launches in issue order), ``r.unchecked`` (C ABI launches
+    that bypass the front ends: (name, kernels, traced names)) and ``r.calls`` (every C ABI call made outside a front end, as a ``Call``;
+    the pointers named in ``BY_VALUE`` replaced by a copy of what they point to).  ``family`` labels the records; ``captured_only`` passes
+    launches outside a graph capture straight through (UnetGraph's eager warm-up).  ``unattributed`` collects traced kernel names that no
+    record or listed launch accounts for.
 
     ``sampler=True`` records the sampler's update launches (``PLMS_CALLS``) only and passes everything else through.  Their operands are
     raw pointers; ``_lib.fptr`` is wrapped to map each pointer back to the tensor it came from, and every operand is cloned right after
@@ -169,6 +200,7 @@ class Recorder:
         self.sampler = sampler
         self.recs: List[Rec] = []
         self.unchecked = []
+        self.calls: List[Call] = []
         self.unattributed = []
         self.depth = 0
         self._names_len = 0
@@ -207,9 +239,16 @@ class Recorder:
 
     def __enter__(self):
         from sparsefusion_b200 import _lib as lib, ops
+        # torch.cuda.graph does not collect garbage before a capture, so the cyclic collector may free an earlier evaluation's CUDA
+        # graphs inside one, which invalidates the capture; the recorder's own allocations make a collection inside a capture likely.
+        # Collect here, outside any capture, and hold the collector off until __exit__, which frees what accumulated meanwhile.
+        gc.collect()
+        self._gc_was_enabled = gc.isenabled()
+        gc.disable()
         self.saved = {} if self.sampler else {n: getattr(ops, n) for n in FRONT_ENDS}
         self.lib_call, self.lib_fptr = lib.call, lib.fptr
         specs = _specs()
+        params = c_params()
         rec = self
         if self.trace:
             self._tbuf = torch.zeros(65, dtype=torch.int64, device='cuda')
@@ -257,7 +296,9 @@ class Recorder:
                 if name == 'conv2d_nhwc':
                     out = outputs['out']
                     # an arena slice: pre-zeroed once per evaluation, reduced into in accumulate mode (linear_tc passes it as ``out``)
-                    r.s['arena'] = in_arena or (pre is None and isinstance(arena, ops.ZeroArena) and storage_of(out) == storage_of(arena.buf))
+                    took_arena = pre is None and isinstance(arena, ops.ZeroArena) and storage_of(out) == storage_of(arena.buf)
+                    r.s['arena'] = in_arena or took_arena
+                    r.s['accumulate'] = scal['accumulate'] or took_arena      # the flag the kernel ran with
                     if prefill is not None:
                         t['prefill'] = prefill
                         r.orig['prefill'] = prefill
@@ -286,6 +327,11 @@ class Recorder:
                 return
             if rec.depth or (rec.captured_only and not torch.cuda.is_current_stream_capturing()):
                 return rec.lib_call(name, *args)
+            a = dict(zip(params[name], args))
+            for k, n in BY_VALUE.items():
+                if a.get(k) is not None:
+                    a[k] = device_floats(a[k], n(a))
+            rec.calls.append(Call(name, a, rec.family, len(rec.recs)))
             rec._snapshot_pointers([p for p in args if isinstance(p, int) and p > (1 << 32)])
             rec._pending()
             n0 = ops.launch_count()
@@ -337,6 +383,9 @@ class Recorder:
         for n, f in self.saved.items():
             setattr(ops, n, f)
         lib.call, lib.fptr = self.lib_call, self.lib_fptr
+        if self._gc_was_enabled:
+            gc.enable()
+        gc.collect()
         if self.trace:
             if not self.sampler:
                 self._pending()
@@ -354,6 +403,45 @@ def _label():
         return '?'
     name = f.f_locals.get('name', f.f_locals.get('pfx', ''))
     return f'{os.path.basename(f.f_code.co_filename)}:{f.f_code.co_name}' + (f'({name})' if isinstance(name, str) and name else '')
+
+
+# ------------------------------------------------------------------------------------------------ replay catalogues
+class Catalogue:
+    """the ``rec(family)`` that oracle/model_runs enters around each family, building a replay test's catalogue: per family a
+    ``Recorder(family, trace=False)``; on exit its records and calls, in issue order, go through ``entry`` (a dict of the launch's
+    geometry and scalars with its family and label, or None for a launch the test does not replay), equal entries are counted in
+    ``calls``, and the records are dropped, so no family's tensors stay alive while the next one runs.  ``entries``: key -> entry, in
+    order of first appearance."""
+
+    def __init__(self, entry):
+        self.entry = entry
+        self.entries = {}
+        self.family = None
+
+    def __call__(self, family):
+        self.family = family
+        return self
+
+    def __enter__(self):
+        self.rec = Recorder(self.family, trace=False).__enter__()
+        return self
+
+    def __exit__(self, *exc):
+        rec, self.rec = self.rec, None
+        rec.__exit__(*exc)
+        torch.cuda.synchronize()
+        self.add(rec.recs, rec.calls)
+        return False
+
+    def add(self, recs: List[Rec], calls: List[Call]) -> None:
+        # a call made after the first ``at`` records sorts between record at - 1 and record at
+        issued = sorted([(i + 0.5, r) for i, r in enumerate(recs)] + [(c.at, c) for c in calls], key=lambda p: p[0])
+        for _, r in issued:
+            e = self.entry(r)
+            if e is None:
+                continue
+            key = tuple(sorted((k, v) for k, v in e.items() if k != 'label'))
+            self.entries.setdefault(key, dict(e, calls=0))['calls'] += 1
 
 
 # ------------------------------------------------------------------------------------------------ poison

@@ -20,6 +20,9 @@ An ulp of a normal fp32 result is at most 2^-23 of its magnitude.
 
 ``emulate_*`` evaluate the kernels' arithmetic in fp32 (torch on the CPU) in their fold orders, with switches that inject single defects; the
 host tests use them to show what the bounds see.
+
+``entry`` turns an oracle/insitu record of a front end, or a call of an LPIPS entry point, into the geometry and memory layout
+tests/test_simt_fp64_gpu.py replays.
 """
 from __future__ import annotations
 
@@ -29,10 +32,14 @@ from typing import Dict, Optional
 import torch
 import torch.nn.functional as F
 
+from .conv_fp64 import nhwc_meta, rows_meta, same_ptr
 from .field_fp64 import ATOL, U32 as U, gamma
 
 ULP = 2.0 ** -23          # one ulp of a normal fp32 value, relative to it
 TF32_HALF = 2.0 ** -11    # cvt.rna.tf32.f32
+LPIPS_NAMES = {'sfb_lpips_prep': 'lpips_prep', 'sfb_lpips_prep_backward': 'lpips_prep_backward', 'sfb_relu_nhwc': 'relu',
+               'sfb_maxpool2x2_nhwc': 'maxpool', 'sfb_maxpool2x2_relu_backward_nhwc': 'maxpool_bwd', 'sfb_add_relu_mask': 'add_relu_mask',
+               'sfb_lpips_head': 'lpips_head'}
 
 
 def expf_fast_rel(x: torch.Tensor) -> torch.Tensor:
@@ -626,3 +633,90 @@ def ref_lpips_prep_backward(gx, normalize, factor):
     sc = torch.tensor([_f32(s) for s in LPIPS_SCALE], dtype=torch.float64, device=gx.device)
     y = (gx.double()[..., :3] * _f32(factor) * (2 if normalize else 1) / sc).permute(2, 0, 1)
     return y, gamma(3) * y.abs() + ATOL
+
+
+# ------------------------------------------------------------------------------------------------ recorded launches
+def _lpips_entry(name, a):
+    if name == 'sfb_lpips_prep':
+        return dict(H=a['H'], W=a['W'], normalize=a['normalize'])
+    if name == 'sfb_lpips_prep_backward':
+        return dict(H=a['H'], W=a['W'], normalize=a['normalize'], factor=float(a['factor']))
+    if name == 'sfb_relu_nhwc':
+        return dict(n=int(a['n']))
+    if name == 'sfb_maxpool2x2_nhwc':
+        return dict(NB=a['NB'], H=a['H'], W=a['W'], C=a['C'])
+    if name == 'sfb_maxpool2x2_relu_backward_nhwc':
+        return dict(H=a['H'], W=a['W'], C=a['C'])
+    if name == 'sfb_add_relu_mask':
+        return dict(n=int(a['n']), head=a['g_head'] is not None)
+    return dict(HW=a['HW'], C=a['C'])                                          # sfb_lpips_head
+
+
+def _front_end_entry(op, t, s):
+    if op == 'groupnorm':
+        x, y, film = t['x'], t['out'], t['film']
+        nb, h, w, c, ldx, xoff = nhwc_meta(x)
+        _, _, _, _, ldy, yoff = nhwc_meta(y)
+        return dict(NB=nb, H=h, W=w, C=c, G=s['groups'], ldx=ldx, xoff=xoff, ldy=ldy, yoff=yoff, film=film is not None,
+                    ldf=film.stride(0) if film is not None else 0, act=s['silu'], alias='x=out' if same_ptr(x, y) else '')
+    if op == 'layernorm':
+        res = t['residual']
+        T, C, ldx, xoff = rows_meta(t['x'])
+        return dict(T=T, C=C, ldx=ldx, xoff=xoff, ldy=rows_meta(t['out'])[2], b=t['b'] is not None, res=res is not None,
+                    ldr=rows_meta(res)[2] if res is not None else 0, pre_gelu=s['pre_gelu'], round=s['round'],
+                    alias='res=out' if same_ptr(res, t['out']) else '')
+    if op == 'linear_small':
+        res = t['residual']
+        M, K, ldx, xoff = rows_meta(t['x'])
+        return dict(M=M, K=K, O=t['w'].shape[0], ldx=ldx, xoff=xoff, ldy=rows_meta(t['out'])[2], bias=t['bias'] is not None,
+                    res=res is not None, ldr=rows_meta(res)[2] if res is not None else 0, pre=s['pre'], post=s['post'], round=s['round'])
+    if op == 'mq_attention':
+        q, ckv = t['q'], t['ckv']
+        return dict(B=q.shape[0], n=q.shape[1], heads=s['heads'], dh=s['dh'], nc=0 if ckv is None else ckv.shape[1])
+    if op == 'cross_attention':
+        q = t['q']
+        return dict(B=q.shape[0], n=q.shape[1], heads=s['heads'], dh=s['dh'], nc=t['kvc'].shape[1])
+    if op == 'gca_pool':
+        nb, h, w, c, ldx, xoff = nhwc_meta(t['x'])
+        return dict(NB=nb, HW=h * w, C=c, ldx=ldx, xoff=xoff)
+    if op == 'gate_mlp_residual':
+        nb, hh, ww, c, ldh, _ = nhwc_meta(t['h'])
+        return dict(NB=nb, HW=hh * ww, C=c, Hd=t['hid'].shape[-1], ldh=ldh, ldr=nhwc_meta(t['res'])[4])
+    if op == 'gate_residual':
+        nb, hh, ww, c, ldh, _ = nhwc_meta(t['h'])
+        return dict(NB=nb, HW=hh * ww, C=c, ldh=ldh, ldr=nhwc_meta(t['res'])[4], ldo=nhwc_meta(t['out'])[4], gate=t['gate'] is not None)
+    if op == 'softmax_rows':
+        r, c, ldx, _ = rows_meta(t['x'])
+        return dict(rows=r, cols=c, ldx=ldx, ldy=rows_meta(t['out'])[2], scale=s['scale'])
+    if op == 'upsample2x':
+        nb, h, w, c, ldx, _ = nhwc_meta(t['x'])
+        return dict(NB=nb, H=h, W=w, C=c, ldx=ldx)
+    if op == 'nchw_to_nhwc':
+        nb, c, h, w = t['src'].shape
+        return dict(NB=nb, C=c, H=h, W=w, ld=nhwc_meta(t['out'])[4], c_off=s['c_off'], round=s['round'])
+    if op == 'nhwc_to_nchw':
+        nb, h, w, c, ld, _ = nhwc_meta(t['src'])
+        return dict(NB=nb, C=c, H=h, W=w, ld=ld)
+    if op == 'im2col4':
+        nb, h, w, c, ldx, _ = nhwc_meta(t['x'])
+        return dict(NB=nb, H=h, W=w, KH=s['kh'], KW=s['kw'], pad=s['pad'], ldx=ldx)
+    if op == 'concat2':
+        nb, h, w, c1, lda, _ = nhwc_meta(t['a'])
+        return dict(NB=nb, H=h, W=w, C1=c1, lda=lda, C2=t['b'].shape[-1], ldb=nhwc_meta(t['b'])[4], ldo=nhwc_meta(t['out'])[4],
+                    scale_b=s['scale_b'])
+    if op == 'pixel_shuffle_silu':
+        nb, h, w, c4, _, _ = nhwc_meta(t['y'])
+        return dict(NB=nb, H=h, W=w, Co=c4 // 4, ldo=nhwc_meta(t['out'])[4])
+    if op == 'time_fourier':
+        return dict(B=t['t'].shape[0], half=t['w'].shape[0])
+    return None                                                                 # conv2d_nhwc: tests/test_conv_fp64_gpu.py
+
+
+def entry(r) -> Optional[Dict]:
+    """the replay entry of an oracle/insitu record: a front-end record other than the GEMM's, or a ``Call`` of an LPIPS entry point read by
+    parameter name (None for any other launch).  Row strides, slice offsets, the FiLM row stride, residual and aliasing (an output at the
+    address of an input); labelled with the family."""
+    if r.op in LPIPS_NAMES:
+        return dict(_lpips_entry(r.op, r.args), op=LPIPS_NAMES[r.op], family=r.family, label=r.family)
+    f = None if r.op.startswith('sfb_') else _front_end_entry(r.op, r.orig, r.s)       # calls carry the C symbol, records the front end
+    return None if f is None else dict(f, op=r.op, family=r.family, label=r.family)

@@ -479,3 +479,52 @@ def ref_seq_attention(qkv: torch.Tensor, S: int, B: int, E: int, defect: Optiona
         return y.permute(1, 0, 2), torch.zeros_like(y).permute(1, 0, 2)
     y, bnd = _softmax_pv_bound(s, sa, 4 * _ceil_div(E, 128) + 6, v, S)
     return y.permute(1, 0, 2), bnd.permute(1, 0, 2)
+
+
+# ------------------------------------------------------------------------------------------------ recorded launches
+def _floats(a, *names):
+    return tuple(float(a[n]) for n in names)
+
+
+def _nulls(a, *names):
+    return tuple(a[n] is None for n in names)
+
+
+COEFS = ('c0', 'c1', 'c2', 'c3')
+STEP_SCALARS = ('alpha', 'sigma', 'alpha_next', 'c', 'noise_scale')
+LAMBDAS = ('lambda_color', 'lambda_sil', 'lambda_opacity')
+ENTRIES = {
+    'sfb_plms_update': ('plms_update', lambda a: dict(
+        n=int(a['n']), nulls=_nulls(a, 'e1', 'e2', 'e3'), coefs=_floats(a, *COEFS), scalars=_floats(a, *STEP_SCALARS), clip=float(a['clip']),
+        x0_out=a['x0_out'] is not None, e_out=a['e_out'] is not None)),
+    'sfb_plms_update_rows': ('plms_update_rows', lambda a: dict(
+        rows=int(a['rows']), row_len=int(a['row_len']), nulls=_nulls(a, 'e1', 'e2', 'e3'), coefs=_floats(a, *COEFS), clip=float(a['clip']),
+        x0_out=a['x0_out'] is not None, row_scalars=tuple(a['row_scalars'].tolist()))),
+    'sfb_plms_update_rows_cfg': ('plms_update_rows_cfg', lambda a: dict(
+        rows=int(a['rows']), row_len=int(a['row_len']), nulls=_nulls(a, 'e1', 'e2', 'e3'), coefs=_floats(a, *COEFS),
+        cond_scale=float(a['cond_scale']), clip=float(a['clip']), e_out=a['e_out'] is not None, row_scalars=tuple(a['row_scalars'].tolist()))),
+    'sfb_photometric_loss': ('photometric_loss', lambda a: dict(h=a['h'], w=a['w'], scale=a['scale'], lam=_floats(a, *LAMBDAS))),
+    'sfb_upsample2x_render': ('upsample2x_render', lambda a: dict(h=a['h'], w=a['w'])),
+    'sfb_fusion_loss_ex': ('fusion_loss', lambda a: dict(h=a['h'], w=a['w'], mode=a['mode'], g_extra=a['g_extra'] is not None,
+                                                         wgt=float(a['weight']), lam=_floats(a, *LAMBDAS))),
+    'sfb_ddpm_dynamic_step': ('ddpm_dynamic_step', lambda a: dict(
+        B=int(a['B']), row_len=int(a['row_len']), guided=a['e_null'] is not None, cond_scale=float(a['cond_scale']),
+        scalars=_floats(a, *STEP_SCALARS), p=float(a['percentile']), s_out=a['s_out'] is not None, x0_out=a['x0_out'] is not None)),
+    'sfb_maxpool3x3s2_nhwc': ('maxpool3x3s2', lambda a: dict(NB=a['NB'], H=a['H'], W=a['W'], C=a['C'])),
+    'sfb_resize_bilinear_ac_nhwc': ('resize', lambda a: dict(NB=a['NB'], H=a['H'], W=a['W'], C=a['C'], Ho=a['Ho'], Wo=a['Wo'], ldx=int(a['ldx']),
+                                                             ldo=int(a['ldo']))),
+    'sfb_grid_sample_nhwc': ('grid_sample', lambda a: dict(NB=a['NB'], H=a['H'], W=a['W'], C=a['C'], M=int(a['M']), ldx=int(a['ldx']),
+                                                           ldo=int(a['ldo']))),
+    'sfb_seq_attention': ('seq_attention', lambda a: dict(S=a['S'], B=a['B'], E=a['E'])),
+    'sfb_act_inplace': ('act', lambda a: dict(n=int(a['n']), kind=a['kind'])),
+}
+
+
+def entry(r) -> Optional[Dict]:
+    """the replay entry (tests/test_step_fp64_gpu.py) of an oracle/insitu ``Call`` of a sampler update, a distillation loss kernel or an
+    EFT-only kernel, its arguments read by parameter name: geometry, strides, the scalars, each row's five step scalars and which optional
+    pointers are NULL (None for any other launch)"""
+    if r.op not in ENTRIES:
+        return None
+    op, fields = ENTRIES[r.op]
+    return dict(fields(r.args), op=op, family=r.family, label='recorded')

@@ -2,110 +2,38 @@
 
 A module fixture runs the UNet (FULL at 32^2 latents, batch 1 / 2 / 8, precompute_time with 51 rows, precompute_cond +
 forward(cond_features=...); SMALL at 128^2), the full VAE encode + decode at 256^2, PerceptualLoss.value_and_grad at 256^2 and the EFT
-(encode at 256^2, a feature_cache of three views), all on seeded weights, with ``ops.conv2d_nhwc`` wrapped so that every launch's geometry
-and memory layout is recorded (``linear_tc`` calls it through the module globals).  Synthetic entries add what the models do not reach.
+(encode at 256^2, a feature_cache of three views), all on seeded weights, under oracle/insitu.Catalogue, which records every launch's
+geometry and memory layout (``conv_fp64.entry``).  Synthetic entries add what the models do not reach.
 
 Each entry is replayed with fresh operands in its recorded layout, on the default path (3xTF32, variant 2), variant 1 and single-pass TF32,
 with three operand sets -- zero-mean ('randn'), one-signed (the bound is then tight relative to |y|) and 'edges' (exact zeros, powers of
 two, low mantissa words 0x1FFF and 0x1800, per-channel magnitudes 2^-8 .. 2^8) -- and compared per element with
     |y_gpu - y| <= (rho_prod + 2 gamma(n_chain)) conv(|x|, |w|) + gamma(n_epi) A            (oracle/conv_fp64.py)
 Operands sit inside NaN-filled buffers: the channels between a slice and its row stride, and the floats before and after every tensor,
-so a tensor map that reads past Cin, Cout, the last image or a slice shows up as NaN; output channels outside the slice must stay
-bit-identical.  The tracer names every replayed launch, and ``launch_plan`` must name the same kernel.
+so a tensor map that reads past Cin, Cout, the last image or a slice shows up as NaN; every float of the output buffer outside the slice
+(random, NaN in every other one) must stay bit-identical.  The tracer names every replayed launch, and ``launch_plan`` must name the same
+kernel.
 
 Out of scope: ordering hazards between launches, which isolated replays cannot see (tests/test_insitu_fp64_gpu.py checks every launch in
 place), the LPIPS head and prep kernels, and the NGP weight-gradient GEMMs issued from C (tests/test_ngp_field_fp64_gpu.py)."""
-import ctypes
 import math
-import os
-import sys
 from collections import defaultdict
 
 import pytest
 import torch
 
-from oracle import conv_fp64 as cf, model_runs
+from _helpers import Out, Tracer, guarded, release
+from oracle import conv_fp64 as cf, insitu, model_runs
 
 pytestmark = pytest.mark.gpu
 
 PATHS = {'tf32x3': ('tf32x3', 2), 'tf32x3-v1': ('tf32x3', 1), 'tf32': ('tf32', 2)}
 SETS = ('randn', 'one-signed', 'edges')
-GUARD = 256          # NaN floats before and after every buffer (1 KB keeps every tensor 16-byte aligned)
 FIELDS = ('NB', 'H', 'W', 'Cin', 'ldx', 'xoff', 'Cout', 'KH', 'KW', 'stride', 'pad', 'pad_after', 'ldo', 'ooff', 'bias', 'residual', 'ldr',
           'roff', 'accumulate', 'w_split', 'dyn', 'splits', 'bn', 'alias')
 
 
 # ------------------------------------------------------------------------------------------------ catalogue
-def _meta(t):
-    from sparsefusion_b200 import ops
-    nb, h, w, c, ld = ops._nhwc_meta(t)
-    off = t.storage_offset() % ld
-    return nb, h, w, c, ld, (off if off + c <= ld else 0)
-
-
-def _label():
-    f = sys._getframe(2)
-    while f is not None and os.path.basename(f.f_code.co_filename) == 'ops.py':
-        f = f.f_back
-    if f is None:
-        return '?'
-    name = f.f_locals.get('name', f.f_locals.get('pfx', ''))
-    return f'{os.path.basename(f.f_code.co_filename)}:{f.f_code.co_name}' + (f'({name})' if isinstance(name, str) and name else '')
-
-
-class _Recorder:
-    """wraps ops.conv2d_nhwc; entries deduplicated on their signature within a family"""
-
-    def __init__(self):
-        self.entries = {}
-        self.family = None
-
-    def __call__(self, family):
-        self.family = family
-        return self
-
-    def __enter__(self):
-        from sparsefusion_b200 import ops
-        self.orig = orig = ops.conv2d_nhwc
-
-        def rec(x, w_packed, cout, kh, kw, stride=1, pad=0, bias=None, residual=None, out=None, accumulate=False, splits=0, bn=0,
-                pad_after=None, w_split=None, dynamic_weights=False):
-            given = out is not None
-            y = orig(x, w_packed, cout, kh, kw, stride, pad, bias, residual, out, accumulate, splits, bn, pad_after, w_split, dynamic_weights)
-            arena = ops._arena
-            if not given and isinstance(arena, ops.ZeroArena) and y.untyped_storage().data_ptr() == arena.buf.untyped_storage().data_ptr():
-                accumulate = True                       # conv2d_nhwc reduced into a pre-zeroed arena slice
-            nb, h, w, cin, ldx, xoff = _meta(x)
-            _, _, _, _, ldo, ooff = _meta(y)
-            ldr, roff = 0, 0
-            if residual is not None:
-                ldr, roff = _meta(residual)[4:]
-            alias = []
-            for a, b, n in ((x, y, 'x=out'), (residual, y, 'res=out'), (x, residual, 'x=res')):
-                if a is not None and b is not None and a.data_ptr() == b.data_ptr():
-                    alias.append(n)
-            e = dict(NB=nb, H=h, W=w, Cin=cin, ldx=ldx, xoff=xoff, Cout=cout, KH=kh, KW=kw, stride=stride, pad=pad,
-                     pad_after=pad if pad_after is None else pad_after, ldo=ldo, ooff=ooff, bias=bias is not None, residual=residual is not None,
-                     ldr=ldr, roff=roff, accumulate=bool(accumulate), w_split=w_split is not None, dyn=bool(dynamic_weights), splits=splits, bn=bn,
-                     alias=','.join(alias), family=self.family)
-            key = (self.family,) + tuple(e[k] for k in FIELDS)
-            if key not in self.entries:
-                e['label'] = _label()
-                e['calls'] = 0
-                self.entries[key] = e
-            self.entries[key]['calls'] += 1
-            return y
-
-        ops.conv2d_nhwc = rec
-        return self
-
-    def __exit__(self, *exc):
-        from sparsefusion_b200 import ops
-        ops.conv2d_nhwc = self.orig
-        torch.cuda.synchronize()
-        return False
-
-
 def _entry(label, NB, H, W, Cin, Cout, K, stride=1, pad=0, pad_after=None, ldx=None, xoff=0, ldo=None, ooff=0, bias=True, residual=False,
            ldr=None, roff=0, accumulate=False, w_split=False, dyn=False, splits=0, bn=0):
     return dict(NB=NB, H=H, W=W, Cin=Cin, ldx=ldx or Cin, xoff=xoff, Cout=Cout, KH=K, KW=K, stride=stride, pad=pad,
@@ -152,9 +80,9 @@ def _synthetic():
 
 @pytest.fixture(scope='module')
 def catalogue():
-    rec = _Recorder()
-    model_runs.record_models(rec)
-    entries = list(rec.entries.values()) + _synthetic()
+    cat = insitu.Catalogue(cf.entry)
+    model_runs.record_models(cat)
+    entries = list(cat.entries.values()) + _synthetic()
     fam = defaultdict(int)
     for e in entries:
         fam[e['family']] += 1
@@ -199,41 +127,7 @@ def _operands(e, kind, seed):
     return x, w, b, r, pre
 
 
-def _guarded(rows, ld, off, values, outside=None):
-    """flat buffer: GUARD NaN floats, [rows, ld] rows holding ``values`` [rows, width] at channel ``off`` and ``outside`` (default NaN)
-    elsewhere, GUARD NaN floats.  Returns (buffer, [rows, ld] body)"""
-    buf = torch.full((rows * ld + 2 * GUARD,), float('nan'), device='cuda')
-    body = buf[GUARD:GUARD + rows * ld].view(rows, ld)
-    if outside is not None:
-        body.copy_(outside)
-    if values is not None:
-        body[:, off:off + values.shape[-1]] = values.reshape(rows, -1)
-    return buf, body
-
-
-def _flat(t):
-    buf = torch.full((t.numel() + 2 * GUARD,), float('nan'), device='cuda')
-    buf[GUARD:GUARD + t.numel()] = t.reshape(-1)
-    return buf, buf[GUARD:GUARD + t.numel()].view(t.shape)
-
-
 # ------------------------------------------------------------------------------------------------ replay
-class _Tracer:
-    def __init__(self):
-        from sparsefusion_b200 import _lib as lib
-        self.lib = lib
-        self.buf = torch.zeros(65, dtype=torch.int64, device='cuda')
-        self.names = ctypes.create_string_buffer(1 << 12)
-
-    def begin(self):
-        self.lib.call('sfb_trace_begin', self.buf.data_ptr(), 64)
-
-    def end(self):
-        self.lib.load().sfb_trace_names(self.names, len(self.names))
-        self.lib.call('sfb_trace_end')
-        return self.names.value.decode().split('\n')[:-1]
-
-
 def _launch(e, path, ops_in, tracer, sm):
     """one replay of entry e on path with operands (x, w, b, r, pre); returns (got NHWC fp32, guard ok, traced names, plan)"""
     from sparsefusion_b200 import _lib as lib, ops
@@ -243,47 +137,27 @@ def _launch(e, path, ops_in, tracer, sm):
     Ho, Wo = cf.out_size(H, W, e['KH'], e['KW'], e['stride'], e['pad'], e['pad_after'])
     ops.set_precision(precision)
     lib.call('sfb_conv_set_variant', variant)
+    release()
     try:
         if e['dyn']:
             wp = w.reshape(Cout, -1).contiguous()          # an activation: used as it is, in every mode
         else:
             wp = ops.pack_conv_weight(w)                   # rounded to tf32 in single-pass mode
-        _, wpv = _flat(wp)
-        spv = None
-        if e['w_split'] and precision == 'tf32x3':
-            _, spv = _flat(ops.split_packed_weight(wp))
-        _, xb = _guarded(NB * H * W, e['ldx'], e['xoff'], x)
-        xv = xb.view(NB, H, W, e['ldx'])[..., e['xoff']:e['xoff'] + Cin]
-        rows = NB * Ho * Wo
-        g = torch.Generator(device='cuda').manual_seed(rows)
-        outside = torch.randn(rows, e['ldo'], device='cuda', generator=g)
-        outside[:, ::2] = float('nan')                 # stray stores and stray adds both change these bits
-        obuf, ob = _guarded(rows, e['ldo'], e['ooff'], pre, outside)
-        if pre is None:
-            ob[:, e['ooff']:e['ooff'] + Cout] = float('nan')
-        before = obuf.clone()
-        ov = ob.view(NB, Ho, Wo, e['ldo'])[..., e['ooff']:e['ooff'] + Cout]
+        wpv = guarded(wp)
+        spv = guarded(ops.split_packed_weight(wp)) if e['w_split'] and precision == 'tf32x3' else None
+        xv = guarded(x, e['ldx'], e['xoff'])
+        out = Out(NB * Ho * Wo, Cout, e['ldo'], e['ooff'], prefill=pre)
+        ov = out.slot.view(NB, Ho, Wo, Cout)
         rv = None
         if r is not None:
-            if 'res=out' in e['alias']:
-                rv = ov
-            else:
-                _, rb = _guarded(rows, e['ldr'], e['roff'], r)
-                rv = rb.view(NB, Ho, Wo, e['ldr'])[..., e['roff']:e['roff'] + Cout]
-        bv = None if b is None else _flat(b)[1]
+            rv = ov if 'res=out' in e['alias'] else guarded(r, e['ldr'], e['roff'])
+        bv = guarded(b)
         plan = cf.launch_plan(NB, H, W, Cin, Cout, e['KH'], e['KW'], e['stride'], e['pad'], e['pad_after'], e['splits'], e['bn'], precision,
                               variant, spv is not None, sm)
-        tracer.begin()
-        try:
-            ops.conv2d_nhwc(xv, wpv, Cout, e['KH'], e['KW'], e['stride'], e['pad'], bias=bv, residual=rv, out=ov, accumulate=e['accumulate'],
-                            splits=e['splits'], bn=e['bn'], pad_after=e['pad_after'], w_split=spv, dynamic_weights=e['dyn'])
-            torch.cuda.synchronize()
-        finally:
-            names = tracer.end()
-        ba, aa = before.view(torch.int32), obuf.view(torch.int32)
-        guard_ok = (torch.equal(ba[:GUARD], aa[:GUARD]) and torch.equal(ba[-GUARD:], aa[-GUARD:])
-                    and cf.slice_guard_intact(before[GUARD:-GUARD].view(rows, -1), obuf[GUARD:-GUARD].view(rows, -1), e['ooff'], Cout))
-        return ov.clone(), guard_ok, names, plan
+        names = tracer.run(lambda: ops.conv2d_nhwc(xv, wpv, Cout, e['KH'], e['KW'], e['stride'], e['pad'], bias=bv, residual=rv, out=ov,
+                                                   accumulate=e['accumulate'], splits=e['splits'], bn=e['bn'], pad_after=e['pad_after'],
+                                                   w_split=spv, dynamic_weights=e['dyn']))
+        return out.value().view(NB, Ho, Wo, Cout), out.guard_ok(), names, plan
     finally:
         ops.set_precision('tf32x3')
         lib.call('sfb_conv_set_variant', 2)
@@ -311,7 +185,7 @@ def _key(e):
 @pytest.fixture(scope='module')
 def replays(catalogue):
     sm = torch.cuda.get_device_properties(0).multi_processor_count
-    tracer = _Tracer()
+    tracer = Tracer()
     res = dict(fail=[], names=defaultdict(set), features=defaultdict(set), table={}, control=[])
     table = defaultdict(lambda: [0, 0.0, 0.0])
     for n, e in enumerate(catalogue):

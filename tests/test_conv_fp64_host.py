@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import conv_fp64 as cf
+from oracle import conv_fp64 as cf, insitu
 
 SM = 132      # H100 SXM
 
@@ -243,3 +243,43 @@ def test_one_single_pass_chunk_in_a_96_step_chain_is_not_visible():
     got = cf.emulate(x, w, plan, 'tf32x3', b, defect='one_chunk_single_pass')
     assert not cf.violations(got, y, bnd, 1.0).any()
     assert not cf.violations(cf.emulate(x, w, plan, 'tf32x3', b), y, bnd, 1.0).any()
+
+
+# ------------------------------------------------------------------------------------------------ catalogue entries of recorded launches
+def _conv_rec(x, out, residual=None, bias=True, **scalars):
+    """an oracle/insitu record of ops.conv2d_nhwc as the recorder builds it, on CPU tensors"""
+    s = dict(cout=out.shape[-1], kh=3, kw=3, stride=1, pad=1, pad_after=1, splits=0, bn=0, dyn=False, accumulate=False, arena=False)
+    s.update(scalars)
+    t = dict(x=x, w_packed=torch.zeros(s['cout'], 9 * 64), bias=torch.zeros(s['cout']) if bias else None, residual=residual, w_split=None,
+             out=out)
+    return insitu.Rec('conv2d_nhwc', t, ('out',), s, family='UNet', label='unet.py:forward')
+
+
+def test_entry_reads_the_channel_slices_of_x_out_and_the_residual():
+    x, out, res = torch.zeros(2, 6, 6, 40)[..., 8:24], torch.zeros(2, 6, 6, 64)[..., 16:40], torch.zeros(2, 6, 6, 48)[..., 4:28]
+    e = cf.entry(_conv_rec(x, out, res, kh=5, kw=1, stride=2, pad=2, pad_after=0, splits=3, bn=64, dyn=True))
+    assert (e['NB'], e['H'], e['W'], e['Cin'], e['ldx'], e['xoff']) == (2, 6, 6, 16, 40, 8)
+    assert (e['Cout'], e['ldo'], e['ooff'], e['residual'], e['ldr'], e['roff']) == (24, 64, 16, True, 48, 4)
+    assert (e['KH'], e['KW'], e['stride'], e['pad'], e['pad_after'], e['splits'], e['bn'], e['dyn']) == (5, 1, 2, 2, 0, 3, 64, True)
+    assert (e['bias'], e['w_split'], e['accumulate'], e['alias']) == (True, False, False, '')
+    assert (e['family'], e['label']) == ('UNet', 'unet.py:forward')
+    assert cf.entry(_conv_rec(x, out, bias=False))['bias'] is False
+    assert cf.entry(insitu.Rec('groupnorm', {}, (), {})) is None
+
+
+def test_entry_alias_is_the_same_address_not_an_overlap():
+    buf = torch.zeros(1, 4, 4, 48)
+    out = buf[..., 8:32]
+    assert cf.entry(_conv_rec(torch.zeros(1, 4, 4, 16), out, out))['alias'] == 'res=out'
+    assert cf.entry(_conv_rec(torch.zeros(1, 4, 4, 16), out, buf[..., 0:24]))['alias'] == ''          # overlapping, other address
+    x = torch.zeros(1, 4, 4, 24)
+    assert cf.entry(_conv_rec(x, x, x))['alias'] == 'x=out,res=out,x=res'
+
+
+def test_entry_of_a_reduction_into_an_arena_slice():
+    """conv2d_nhwc took its output from the split-K arena: the kernel accumulated into the pre-zeroed slice (``accumulate`` is the flag it
+    ran with), and the slice's offset in the arena is not a channel offset"""
+    arena = torch.zeros(4096)
+    out = arena[64:64 + 4 * 4 * 24].view(1, 4, 4, 24)
+    e = cf.entry(_conv_rec(torch.zeros(1, 4, 4, 16), out, accumulate=True, arena=True))
+    assert (e['accumulate'], e['ldo'], e['ooff']) == (True, 24, 0)

@@ -295,3 +295,21 @@ def test_conv_gemm_kernel_reads_only_bias_tensor_maps_and_weight_stages_before_i
     assert 'tma_load' not in re.sub(r'auto load_(?:weights|acts) = \[&\]\(int it\) \{.*?\n\s*\};', '', pre, flags=re.S)
     # every thread of the epilogue waits before its residual reads and output writes
     assert re.search(r'pdl_wait\(\);\s*(?:\n[^\n]*)*?\bp\.residual', body[first + 1:]) or 'residual' not in body[first + 1:]
+
+
+# ------------------------------------------------------------------------------------------------ replay catalogues
+def test_catalogue_orders_records_and_calls_as_issued_and_counts_repeats():
+    """the replay tests seed each entry's operands by its position, so calls interleave with the front-end records in issue order"""
+    from oracle import simt_fp64 as sf
+    sm = lambda cols: insitu.Rec('softmax_rows', dict(x=torch.zeros(3, cols), out=torch.zeros(3, cols)), ('out',), dict(scale=1.0),
+                                 family='LPIPS')
+    relu = lambda n, at: insitu.Call('sfb_relu_nhwc', dict(x=1, n=n, stream=0), 'LPIPS', at)
+    gemm = insitu.Rec('conv2d_nhwc', {}, (), {}, family='LPIPS')               # not a SIMT entry
+    cat = insitu.Catalogue(sf.entry)
+    # issued: relu 8, softmax 4, gemm, relu 16, softmax 4, relu 8
+    cat.add([sm(4), gemm, sm(4)], [relu(8, 0), relu(16, 2), relu(8, 3)])
+    got = [(e['op'], e.get('n', e.get('cols')), e['calls']) for e in cat.entries.values()]
+    assert got == [('relu', 8, 2), ('softmax_rows', 4, 2), ('relu', 16, 1)], got
+    cat.add([sm(5)], [relu(8, 1)])                                              # a later family run adds to the same catalogue
+    assert [(e['op'], e['calls']) for e in cat.entries.values()][1:] == [('softmax_rows', 2), ('relu', 1), ('softmax_rows', 1)]
+    assert next(iter(cat.entries.values()))['calls'] == 3

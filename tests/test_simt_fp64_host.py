@@ -14,7 +14,7 @@ import math
 import pytest
 import torch
 
-from oracle import simt_fp64 as sf
+from oracle import insitu, simt_fp64 as sf
 
 SM = 132      # H100 SXM
 
@@ -214,3 +214,41 @@ def test_lpips_head_bound_and_epsilon():
     assert abs(float(ev) - float(v)) <= float(vb) and sf.max_ratio(eg, gr, gb) < 1
     dv, dg = sf.emulate_lpips_head(f0, f1, w, 'eps_outside')
     assert not (abs(float(dv) - float(v)) <= float(vb)) or _rejected(dg, gr, gb)
+
+
+# ------------------------------------------------------------------------------------------------ catalogue entries of recorded launches
+def _call(name, *args):
+    """an oracle/insitu ``Call``: positional C ABI arguments bound to the header's parameter names, as the recorder binds them"""
+    return insitu.Call(name, dict(zip(insitu.c_params()[name], args)), 'LPIPS')
+
+
+def test_entry_reads_front_end_slices_strides_and_aliases():
+    rows = torch.zeros(1, 4, 4, 96)
+    x = rows[..., 16:80]
+    film = torch.zeros(1, 192)[:, :128]
+    gn = insitu.Rec('groupnorm', dict(x=x, gamma=torch.zeros(64), beta=torch.zeros(64), film=film, out=x), ('out',),
+                    dict(groups=8, silu=True, eps=1e-5), family='VAE')
+    assert sf.entry(gn) == dict(NB=1, H=4, W=4, C=64, G=8, ldx=96, xoff=16, ldy=96, yoff=16, film=True, ldf=192, act=True, alias='x=out',
+                                op='groupnorm', family='VAE', label='VAE')
+    xs = torch.zeros(5, 48)[:, 8:48]
+    out = torch.zeros(5, 44)[:, :40]
+    ln = insitu.Rec('layernorm', dict(x=xs, g=torch.zeros(40), b=None, residual=out, out=out), ('out',),
+                    dict(pre_gelu=True, round=False), family='EFT')
+    assert sf.entry(ln) == dict(T=5, C=40, ldx=48, xoff=8, ldy=44, b=False, res=True, ldr=44, pre_gelu=True, round=False, alias='res=out',
+                                op='layernorm', family='EFT', label='EFT')
+    dst = torch.zeros(2, 3, 3, 48)
+    nc = insitu.Rec('nchw_to_nhwc', dict(src=torch.zeros(2, 36, 3, 3), out=dst[..., 8:44]), ('out',), dict(round=True, c_off=8), family='UNet')
+    assert sf.entry(nc) == dict(NB=2, C=36, H=3, W=3, ld=48, c_off=8, round=True, op='nchw_to_nhwc', family='UNet', label='UNet')
+    assert sf.entry(insitu.Rec('conv2d_nhwc', {}, (), {})) is None
+
+
+def test_entry_reads_lpips_calls_by_parameter_name():
+    bwd = sf.entry(_call('sfb_maxpool2x2_relu_backward_nhwc', 11, 12, 13, 6, 10, 5, 0))      # x, gy, gx, H, W, C, stream
+    assert bwd == dict(H=6, W=10, C=5, op='maxpool_bwd', family='LPIPS', label='LPIPS')
+    assert sf.entry(_call('sfb_add_relu_mask', 11, None, 13, 4096, 0))['n'] == 4096
+    assert sf.entry(_call('sfb_add_relu_mask', 11, 12, 13, 4096, 0))['head'] is True
+    assert sf.entry(_call('sfb_add_relu_mask', 11, None, 13, 4096, 0))['head'] is False
+    prep = sf.entry(_call('sfb_lpips_prep_backward', 11, 64, 32, 1, 0.25, 12, 0))               # gx, H, W, normalize, factor, g_pred
+    assert (prep['H'], prep['W'], prep['normalize'], prep['factor']) == (64, 32, 1, 0.25)
+    assert sf.entry(_call('sfb_lpips_head', 11, 12, 13, 100, 68, 14, 15, 0))['HW'] == 100
+    assert sf.entry(_call('sfb_seq_attention', 11, 12, 3, 4, 5, 0)) is None

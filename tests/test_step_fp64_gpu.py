@@ -2,8 +2,9 @@
 csrc/eft_ops.cu replayed per element against fp64 (oracle/step_fp64.py).
 
 A module fixture records the launches of DDPM.sample, of PLMSSampler (scene-batched and guided) and of two Distiller steps
-(oracle/model_runs.record_steps), and of the EFT (record_eft), by wrapping ``_lib.call``: geometry, strides, the scalars (alpha, sigma, clip,
-percentile, cond_scale, the coefficients, each row's five step scalars, the loss weights) and which history pointers are NULL.  Synthetic
+(oracle/model_runs.record_steps), and of the EFT (record_eft), under oracle/insitu.Catalogue, which reads each C ABI call's arguments by
+parameter name (``step_fp64.entry``): geometry, strides, the scalars (alpha, sigma, clip, percentile, cond_scale, the coefficients, each
+row's five step scalars, the loss weights) and which history pointers are NULL.  Synthetic
 entries add what the models do not reach: h != w and h or w = 1 in the glue, scale 1 / 2 / 4, mode-1 mask means exactly at 0.1f and one ulp
 either side, d = 0 exactly; row lengths 1, 255, 256, 257, 8192, 8193, 57 345 and 65 536 and one row past 1024 x 256 floats; every pattern of
 NULL history pointers and NULL optional outputs; all |x0| < 1, rank ties that span the cluster's CTAs, +-0 and subnormals, p = 0 and 1;
@@ -12,13 +13,13 @@ E = 4, 132.
 
 Each entry is replayed through the C ABI with the operand sets 'randn', 'one-signed', 'edges' and -- for the kernels whose clamps and maxima
 must keep NaN (the sampler updates, the 3x3 max-pool, ReLU) -- 'non-finite' (NaN and +-inf in eps, x and the activations): NaN positions
-must equal the reference's, other elements are held to the usual bound.  Operands sit in NaN-filled guard buffers; output channels outside
-a slice (resize, grid_sample) and the floats around every output stay bit-identical.  The sampler kernels' traced names must equal the
+must equal the reference's, other elements are held to the usual bound.  Operands sit in NaN-filled guard buffers; every float of an
+output buffer outside the output (random, NaN in every other one: channels outside a slice in resize and grid_sample, the floats around
+every output) stays bit-identical.  The sampler kernels' traced names must equal the
 plan.  Every output except the glue's atomic loss sums must repeat bit for bit.
 
 Out of scope: sfb_eft_t1_tokens (tests/test_scene_gpu.py), sfb_rays_from_camera (bitwise, tests/test_image_glue_gpu.py), NaN grid
 coordinates and ordering hazards between launches."""
-import ctypes
 import math
 from collections import defaultdict
 
@@ -26,92 +27,18 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import model_runs, step_fp64 as sp
+from _helpers import NAN, Out, Tracer, guarded, ptr, release
+from oracle import insitu, model_runs, step_fp64 as sp
 
 pytestmark = pytest.mark.gpu
 
-GUARD = 256
 SETS = ('randn', 'one-signed', 'edges', 'non-finite')
 NONFINITE = {'plms_update', 'plms_update_rows', 'plms_update_rows_cfg', 'ddpm_dynamic_step', 'maxpool3x3s2', 'act'}
-NAN = float('nan')
 PLMS4 = (55 / 24, -59 / 24, 37 / 24, -9 / 24)
 SCAL = (0.8, 0.6, 0.9, 0.3, 0.1)           # alpha, sigma, alpha_next, c, noise_scale
 
 
 # ------------------------------------------------------------------------------------------------ catalogue
-def _device_floats(ptr, n):
-    """a copy of n floats at a device address (the row-scalar tables the row kernels read)"""
-    class _View:
-        __cuda_array_interface__ = dict(shape=(n,), typestr='<f4', data=(ptr, False), version=3)
-    return torch.as_tensor(_View(), device='cuda').clone()
-
-
-class _Recorder:
-    """wraps _lib.call; entries deduplicated on their geometry and scalars within a family"""
-
-    def __init__(self):
-        self.entries = {}
-        self.family = None
-
-    def __call__(self, family):
-        self.family = family
-        return self
-
-    def add(self, op, **f):
-        key = (self.family, op) + tuple(sorted(f.items()))
-        if key not in self.entries:
-            self.entries[key] = dict(f, op=op, family=self.family, label='recorded')
-
-    def __enter__(self):
-        from sparsefusion_b200 import _lib as lib
-        self.lib_call = lib.call
-        rec = self
-
-        def call(name, *a):
-            if name == 'sfb_plms_update':
-                rec.add('plms_update', n=int(a[19]), nulls=tuple(p is None for p in a[2:5]), coefs=tuple(float(v) for v in a[5:9]),
-                        scalars=tuple(float(v) for v in a[10:15]), clip=float(a[15]), x0_out=a[17] is not None, e_out=a[18] is not None)
-            elif name == 'sfb_plms_update_rows':
-                rows = int(a[14])
-                rec.add('plms_update_rows', rows=rows, row_len=int(a[15]), nulls=tuple(p is None for p in a[2:5]),
-                        coefs=tuple(float(v) for v in a[5:9]), clip=float(a[11]), x0_out=a[13] is not None,
-                        row_scalars=tuple(_device_floats(a[10], 5 * rows).tolist()))
-            elif name == 'sfb_plms_update_rows_cfg':
-                rows = int(a[16])
-                rec.add('plms_update_rows_cfg', rows=rows, row_len=int(a[17]), nulls=tuple(p is None for p in a[4:7]),
-                        coefs=tuple(float(v) for v in a[7:11]), cond_scale=float(a[3]), clip=float(a[13]), e_out=a[15] is not None,
-                        row_scalars=tuple(_device_floats(a[12], 5 * rows).tolist()))
-            elif name == 'sfb_photometric_loss':
-                rec.add('photometric_loss', h=a[4], w=a[5], scale=a[6], lam=tuple(float(v) for v in a[7:10]))
-            elif name == 'sfb_upsample2x_render':
-                rec.add('upsample2x_render', h=a[2], w=a[3])
-            elif name == 'sfb_fusion_loss_ex':
-                rec.add('fusion_loss', h=a[12], w=a[13], mode=a[4], g_extra=a[9] is not None, wgt=float(a[5]), lam=tuple(float(v) for v in a[6:9]))
-            elif name == 'sfb_ddpm_dynamic_step':
-                rec.add('ddpm_dynamic_step', B=int(a[12]), row_len=int(a[11]), guided=a[2] is not None, cond_scale=float(a[3]),
-                        scalars=tuple(float(v) for v in a[5:10]), p=float(a[10]), s_out=a[14] is not None, x0_out=a[15] is not None)
-            elif name == 'sfb_maxpool3x3s2_nhwc':
-                rec.add('maxpool3x3s2', NB=a[2], H=a[3], W=a[4], C=a[5])
-            elif name == 'sfb_resize_bilinear_ac_nhwc':
-                rec.add('resize', NB=a[4], H=a[5], W=a[6], C=a[7], Ho=a[8], Wo=a[9], ldx=int(a[1]), ldo=int(a[3]))
-            elif name == 'sfb_grid_sample_nhwc':
-                rec.add('grid_sample', NB=a[5], H=a[6], W=a[7], C=a[8], M=int(a[9]), ldx=int(a[1]), ldo=int(a[4]))
-            elif name == 'sfb_seq_attention':
-                rec.add('seq_attention', S=a[2], B=a[3], E=a[4])
-            elif name == 'sfb_act_inplace':
-                rec.add('act', n=int(a[1]), kind=a[2])
-            return rec.lib_call(name, *a)
-
-        lib.call = call
-        return self
-
-    def __exit__(self, *exc):
-        from sparsefusion_b200 import _lib as lib
-        lib.call = self.lib_call
-        torch.cuda.synchronize()
-        return False
-
-
 def _plms(label, n, nulls=(False, False, False), x0_out=True, e_out=True, clip=1.0, scalars=SCAL, coefs=PLMS4):
     return dict(op='plms_update', n=n, nulls=nulls, coefs=coefs, scalars=scalars, clip=clip, x0_out=x0_out, e_out=e_out, label=label)
 
@@ -185,10 +112,10 @@ def _synthetic():
 
 @pytest.fixture(scope='module')
 def catalogue():
-    rec = _Recorder()
-    model_runs.record_steps(rec)
-    model_runs.record_eft(rec)
-    entries = list(rec.entries.values()) + _synthetic()
+    cat = insitu.Catalogue(sp.entry)
+    model_runs.record_steps(cat)
+    model_runs.record_eft(cat)
+    entries = list(cat.entries.values()) + _synthetic()
     fam = defaultdict(int)
     for e in entries:
         fam[(e['family'], e['op'])] += 1
@@ -196,7 +123,7 @@ def catalogue():
     return entries
 
 
-# ------------------------------------------------------------------------------------------------ operands and guarded buffers
+# ------------------------------------------------------------------------------------------------ operands
 class _Gen:
     def __init__(self, kind, seed):
         self.kind = kind
@@ -220,64 +147,8 @@ class _Gen:
         return torch.rand(*shape, device='cuda', generator=self.g)
 
 
-_ALIVE = []
-
-
-def _in(t):
-    """pointer to ``t`` inside a NaN buffer [GUARD | t | GUARD] (None passes through)"""
-    if t is None:
-        return None
-    buf = torch.full((t.numel() + 2 * GUARD,), NAN, device='cuda')
-    buf[GUARD:GUARD + t.numel()] = t.reshape(-1).float()
-    _ALIVE.append(buf)
-    return buf[GUARD:].data_ptr()
-
-
-class _Out:
-    """rows x ld floats with the result at channel ``off`` (width floats per row), between GUARD floats; every float outside the result
-    random with NaN in every other one, the result NaN before the launch"""
-
-    def __init__(self, rows, width, ld=None, off=0, seed=0):
-        ld = ld or width
-        g = torch.Generator(device='cuda').manual_seed(seed + rows * 7 + ld)
-        self.rows, self.ld, self.off, self.width = rows, ld, off, width
-        self.buf = torch.randn(rows * ld + 2 * GUARD, device='cuda', generator=g)
-        self.buf[::2] = NAN
-        self.body = self.buf[GUARD:GUARD + rows * ld].view(rows, ld)
-        self.body[:, off:off + width] = NAN
-        self.before = self.buf.clone()
-        self.ptr = self.body[:, off:].data_ptr()
-        _ALIVE.append(self.buf)
-
-    def value(self):
-        return self.body[:, self.off:self.off + self.width].clone()
-
-    def guard_ok(self):
-        keep = torch.ones_like(self.buf, dtype=torch.bool)
-        keep[GUARD:GUARD + self.rows * self.ld].view(self.rows, self.ld)[:, self.off:self.off + self.width] = False
-        return torch.equal(self.before.view(torch.int32)[keep], self.buf.view(torch.int32)[keep])
-
-
 def _opt(flag, rows, width, seed):
-    return _Out(rows, width, seed=seed) if flag else None
-
-
-class _Tracer:
-    def __init__(self):
-        from sparsefusion_b200 import _lib as lib
-        self.lib = lib
-        self.buf = torch.zeros(65, dtype=torch.int64, device='cuda')
-        self.names = ctypes.create_string_buffer(1 << 12)
-
-    def run(self, fn):
-        self.lib.call('sfb_trace_begin', self.buf.data_ptr(), 64)
-        try:
-            fn()
-            torch.cuda.synchronize()
-        finally:
-            self.lib.load().sfb_trace_names(self.names, len(self.names))
-            self.lib.call('sfb_trace_end')
-        return self.names.value.decode().split('\n')[:-1]
+    return Out(rows, width, seed=seed) if flag else None
 
 
 def _row_scalars(rows):
@@ -293,7 +164,7 @@ def _replay(e, kind, seed, tracer, sm):
     from sparsefusion_b200 import _lib as lib
     G = _Gen(kind, seed)
     op = e['op']
-    _ALIVE.clear()
+    release()
     call, S = lib.call, lib.stream()
     res = dict(checks=[], flags=[], guard=True, names=None, planned=None, again=True)
     outs = []
@@ -322,9 +193,9 @@ def _replay(e, kind, seed, tracer, sm):
             sc = torch.tensor(e['scalars'], dtype=torch.float32).view(1, 5)
         else:
             sc = torch.tensor(e['row_scalars']).view(rows, 5) if 'row_scalars' in e else _row_scalars(rows)
-        ptrs = [_in(t) for t in eps]
-        xp, zp = _in(x), _in(noise)
-        xo = _Out(rows, L, seed=1)
+        ptrs = [ptr(guarded(t)) for t in eps]
+        xp, zp = ptr(guarded(x)), ptr(guarded(noise))
+        xo = Out(rows, L, seed=1)
         outs.append(xo)
         if op == 'plms_update':
             x0o, eo = _opt(e['x0_out'], 1, L, 2), _opt(e['e_out'], 1, L, 3)
@@ -350,7 +221,7 @@ def _replay(e, kind, seed, tracer, sm):
             if eo:
                 chk('e', got[k], r['e'])
         elif op == 'plms_update_rows':
-            scp = _in(sc)
+            scp = ptr(guarded(sc))
             x0o = _opt(e['x0_out'], rows, L, 2)
             if x0o:
                 outs.append(x0o)
@@ -364,9 +235,7 @@ def _replay(e, kind, seed, tracer, sm):
             for rr in range(0, rows, max(1, rows - 1)):
                 o1 = torch.full((L,), NAN, device='cuda')
                 rp = [None if t is None else t[rr].contiguous() for t in eps]
-                _ALIVE.extend(t for t in rp if t is not None)
                 xr, zr = x[rr].contiguous(), noise[rr].contiguous()
-                _ALIVE.extend((xr, zr, o1))
                 call('sfb_plms_update', xr.data_ptr(), *[None if t is None else t.data_ptr() for t in rp], *coefs, zr.data_ptr(),
                      *[float(v) for v in sc[rr]], e['clip'], o1.data_ptr(), None, None, L, S)
                 torch.cuda.synchronize()
@@ -374,7 +243,7 @@ def _replay(e, kind, seed, tracer, sm):
         else:
             en = G(rows, L, scale=0.7)
             ec = eps[0]
-            enp, scp = _in(en), _in(sc)
+            enp, scp = ptr(guarded(en)), ptr(guarded(sc))
             eo = _opt(e['e_out'], rows, L, 3)
             if eo:
                 outs.append(eo)
@@ -426,8 +295,8 @@ def _replay(e, kind, seed, tracer, sm):
                     en[1, L // 5] = math.inf
                 if L > 1:
                     x[1, 0] = -math.inf
-        xp, cp, np_, zp = _in(x), _in(ec), _in(en), _in(noise)
-        xo, so, x0o = _Out(B, L, seed=1), _Out(1, B, seed=2), _Out(B, L, seed=3)
+        xp, cp, np_, zp = ptr(guarded(x)), ptr(guarded(ec)), ptr(guarded(en)), ptr(guarded(noise))
+        xo, so, x0o = Out(B, L, seed=1), Out(1, B, seed=2), Out(B, L, seed=3)
         outs += [xo, so, x0o]
         cs = e['cond_scale']
         args = lambda xo_, so_, x0_: (xp, cp, np_, cs, zp, al, sg, an, c, ns, e['p'], L, B, xo_, so_, x0_, S)
@@ -444,7 +313,7 @@ def _replay(e, kind, seed, tracer, sm):
         if pat == 'small' and kind != 'non-finite':                   # the non-finite set puts a NaN in row 0
             res['flags'].append(('s = 1', bool((s_got == 1).all())))
         if not (e['s_out'] and e['x0_out']):                           # the entry's own NULL outputs: the same x_prev
-            o2 = _Out(B, L, seed=4)
+            o2 = Out(B, L, seed=4)
             call('sfb_ddpm_dynamic_step', *args(o2.ptr, so.ptr if e['s_out'] else None, x0o.ptr if e['x0_out'] else None))
             torch.cuda.synchronize()
             res['flags'].append(('NULL outputs leave x_prev unchanged', torch.equal(o2.value().view(torch.int32), got[0].view(torch.int32))))
@@ -461,8 +330,8 @@ def _replay(e, kind, seed, tracer, sm):
         elif kind == 'one-signed':
             img = img + 1.0
         lam = e['lam']
-        ip, sp_, rp, mp = _in(img), _in(sil), _in(rgb), _in(mask)
-        so, gi, gs = _Out(1, 3, seed=1), _Out(n, 3, seed=2), _Out(1, n, seed=3)
+        ip, sp_, rp, mp = ptr(guarded(img)), ptr(guarded(sil)), ptr(guarded(rgb)), ptr(guarded(mask))
+        so, gi, gs = Out(1, 3, seed=1), Out(n, 3, seed=2), Out(1, n, seed=3)
         outs += [so, gi, gs]
         got = run(lambda: call('sfb_photometric_loss', ip, sp_, rp, mp, h, w, scl, *lam, so.ptr, gi.ptr, gs.ptr, S), repeat=False)
         # the repeat: gradients only (the sums are atomics)
@@ -477,9 +346,9 @@ def _replay(e, kind, seed, tracer, sm):
     elif op == 'upsample2x_render':
         h, w = e['h'], e['w']
         img, sil = G(h * w, 3), G(h * w)
-        up = _Out(1, 16 * h * w)
+        up = Out(1, 16 * h * w)
         outs.append(up)
-        got = run(lambda: call('sfb_upsample2x_render', _in(img), _in(sil), h, w, up.ptr, S))
+        got = run(lambda: call('sfb_upsample2x_render', ptr(guarded(img)), ptr(guarded(sil)), h, w, up.ptr, S))
         chk('up', got[0].view(4, 2 * h, 2 * w), sp.ref_upsample2x(img, sil, h, w))
     elif op == 'fusion_loss':
         h, w, mode = e['h'], e['w'], e['mode']
@@ -502,8 +371,8 @@ def _replay(e, kind, seed, tracer, sm):
             up[:3] += 1.0
         ge = G(3, H, W, scale=1e-4) if e['g_extra'] else None
         lam = e['lam']
-        upp, tp, gep = _in(up), _in(target), _in(ge)
-        so, gu, gi, gs = _Out(1, 3, seed=1), _Out(1, 4 * HW, seed=2), _Out(h * w, 3, seed=3), _Out(1, h * w, seed=4)
+        upp, tp, gep = ptr(guarded(up)), ptr(guarded(target)), ptr(guarded(ge))
+        so, gu, gi, gs = Out(1, 3, seed=1), Out(1, 4 * HW, seed=2), Out(h * w, 3, seed=3), Out(1, h * w, seed=4)
         outs += [so, gu, gi, gs]
         fn = lambda: call('sfb_fusion_loss_ex', upp, tp, H, W, mode, e['wgt'], *lam, gep, so.ptr, gu.ptr, h, w, gi.ptr, gs.ptr, S)
         got = run(fn, repeat=False)
@@ -523,24 +392,21 @@ def _replay(e, kind, seed, tracer, sm):
         if kind == 'edges':
             x = torch.round(x).clamp(-1, 2) + 0.0                      # ties
         Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
-        y = _Out(1, NB * Ho * Wo * C)
+        y = Out(1, NB * Ho * Wo * C)
         outs.append(y)
-        got = run(lambda: call('sfb_maxpool3x3s2_nhwc', _in(x), y.ptr, NB, H, W, C, S))
+        got = run(lambda: call('sfb_maxpool3x3s2_nhwc', ptr(guarded(x)), y.ptr, NB, H, W, C, S))
         chk('y', got[0].view(NB, Ho, Wo, C), (sp.maxpool3x3s2(x.cpu()), None))
     elif op == 'act':
         n, k = e['n'], e['kind']
         x = G(n, scale=3.0)
-        buf = torch.full((n + 2 * GUARD,), NAN, device='cuda')
-        buf[GUARD:GUARD + n] = x
-        _ALIVE.append(buf)
-        before = buf.clone()
-        tracer.run(lambda: call('sfb_act_inplace', buf[GUARD:].data_ptr(), n, k, S))
-        got = buf[GUARD:GUARD + n].clone()
-        res['guard'] = torch.equal(before[:GUARD].view(torch.int32), buf[:GUARD].view(torch.int32)) and torch.equal(before[-GUARD:].view(torch.int32), buf[-GUARD:].view(torch.int32))
-        buf[GUARD:GUARD + n] = x
-        call('sfb_act_inplace', buf[GUARD:].data_ptr(), n, k, S)
+        o = Out(1, n, prefill=x)                                       # in place
+        tracer.run(lambda: call('sfb_act_inplace', o.ptr, n, k, S))
+        got = o.value().view(n)
+        res['guard'] = o.guard_ok()
+        o.slot[:] = x.view(1, n)
+        call('sfb_act_inplace', o.ptr, n, k, S)
         torch.cuda.synchronize()
-        res['again'] = torch.equal(got.view(torch.int32), buf[GUARD:GUARD + n].view(torch.int32))
+        res['again'] = torch.equal(got.view(torch.int32), o.value().view(n).view(torch.int32))
         chk('relu' if k == 0 else 'gelu', got, (sp.relu(x.cpu()), None) if k == 0 else sp.ref_gelu(x))
     elif op == 'resize':
         NB, H, W, C, Ho, Wo, ldx, ldo = e['NB'], e['H'], e['W'], e['C'], e['Ho'], e['Wo'], e['ldx'], e['ldo']
@@ -548,9 +414,9 @@ def _replay(e, kind, seed, tracer, sm):
         x = G(NB, H, W, C)
         xb = torch.full((NB * H * W, ldx), NAN, device='cuda')
         xb[:, :C] = x.view(-1, C)
-        y = _Out(NB * Ho * Wo, C, ld=ldo, off=off)
+        y = Out(NB * Ho * Wo, C, ld=ldo, off=off)
         outs.append(y)
-        got = run(lambda: call('sfb_resize_bilinear_ac_nhwc', _in(xb), ldx, y.ptr, ldo, NB, H, W, C, Ho, Wo, S))
+        got = run(lambda: call('sfb_resize_bilinear_ac_nhwc', ptr(guarded(xb)), ldx, y.ptr, ldo, NB, H, W, C, Ho, Wo, S))
         chk('y', got[0].view(NB, Ho, Wo, C), sp.ref_resize(x, Ho, Wo))
     elif op == 'grid_sample':
         NB, H, W, C, M, ldx, ldo = e['NB'], e['H'], e['W'], e['C'], e['M'], e['ldx'], e['ldo']
@@ -566,16 +432,16 @@ def _replay(e, kind, seed, tracer, sm):
             g0 = grid[0]
             special = torch.stack((torch.stack((cx, cy), -1), torch.sign(g0), g0 * 3), 0)
             grid = special[k % 3, k].expand(NB, M, 2).contiguous()
-        y = _Out(NB * M, C, ld=ldo, off=off)
+        y = Out(NB * M, C, ld=ldo, off=off)
         outs.append(y)
-        got = run(lambda: call('sfb_grid_sample_nhwc', _in(xb), ldx, _in(grid), y.ptr, ldo, NB, H, W, C, M, S))
+        got = run(lambda: call('sfb_grid_sample_nhwc', ptr(guarded(xb)), ldx, ptr(guarded(grid)), y.ptr, ldo, NB, H, W, C, M, S))
         chk('out', got[0].view(NB, M, C), sp.ref_grid_sample(x, grid))
     elif op == 'seq_attention':
         S_, B, E_ = e['S'], e['B'], e['E']
         qkv = G(S_, B, 3 * E_, scale=(4.0 / math.sqrt(math.sqrt(E_))) if kind == 'edges' else 1.0)
-        y = _Out(1, S_ * B * E_)
+        y = Out(1, S_ * B * E_)
         outs.append(y)
-        got = run(lambda: call('sfb_seq_attention', _in(qkv), y.ptr, S_, B, E_, S))
+        got = run(lambda: call('sfb_seq_attention', ptr(guarded(qkv)), y.ptr, S_, B, E_, S))
         chk('out', got[0].view(S_, B, E_), sp.ref_seq_attention(qkv, S_, B, E_))
     else:
         raise KeyError(op)
@@ -610,7 +476,7 @@ def _key(e):
 @pytest.fixture(scope='module')
 def replays(catalogue):
     sm = torch.cuda.get_device_properties(0).multi_processor_count
-    tracer = _Tracer()
+    tracer = Tracer()
     out = dict(fail=[], names=set(), table={}, runs=0)
     table = {}
     for n, e in enumerate(catalogue):

@@ -13,7 +13,7 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from oracle import step_fp64 as sp
+from oracle import insitu, step_fp64 as sp
 
 SM = 132      # H100 SXM
 g = torch.Generator().manual_seed(0)
@@ -268,3 +268,40 @@ def test_eft_defects():
     assert sp.passes(fp32, y, b)
     for defect in ('scale_1_over_E', 'softmax_over_batch'):
         assert not sp.passes(sp.ref_seq_attention(qkv, S, B, E, defect)[0].float(), y, b), defect
+
+
+# ------------------------------------------------------------------------------------------------ catalogue entries of recorded launches
+def _call(name, *args, family='Distill'):
+    """an oracle/insitu ``Call``: positional C ABI arguments bound to the header's parameter names, as the recorder binds them"""
+    return insitu.Call(name, dict(zip(insitu.c_params()[name], args)), family)
+
+
+def test_entry_reads_sampler_calls_by_parameter_name():
+    # x, e0, e1, e2, e3, c0..c3, noise, alpha, sigma, alpha_next, c, noise_scale, clip, x_prev, x0_out, e_out, n, stream
+    e = sp.entry(_call('sfb_plms_update', 1, 2, None, 4, None, 0.5, 1.5, 2.5, 3.5, 10, 0.8, 0.6, 0.9, 0.3, 0.1, 7.0, 20, None, 22, 4096, 0,
+                       family='DDPM'))
+    assert e == dict(n=4096, nulls=(True, False, True), coefs=(0.5, 1.5, 2.5, 3.5), scalars=(0.8, 0.6, 0.9, 0.3, 0.1), clip=7.0,
+                     x0_out=False, e_out=True, op='plms_update', family='DDPM', label='recorded')
+    # x, e_cond, e_null, cond_scale, e1, e2, e3, c0..c3, noise, row_scalars (copied at call time), clip, x_prev, e_out, rows, row_len, stream
+    table = torch.arange(10, dtype=torch.float32) / 16
+    e = sp.entry(_call('sfb_plms_update_rows_cfg', 1, 2, 3, 3.0, 5, None, None, 0.5, 1.5, 2.5, 3.5, 12, table, 1.0, 15, None, 2, 8192, 0,
+                       family='PLMS'))
+    assert e == dict(rows=2, row_len=8192, nulls=(False, True, True), coefs=(0.5, 1.5, 2.5, 3.5), cond_scale=3.0, clip=1.0, e_out=False,
+                     row_scalars=tuple(table.tolist()), op='plms_update_rows_cfg', family='PLMS', label='recorded')
+    # x, e_cond, e_null, cond_scale, noise, alpha, sigma, alpha_next, c, noise_scale, percentile, row_len, B, x_prev, s_out, x0_out, stream
+    e = sp.entry(_call('sfb_ddpm_dynamic_step', 1, 2, None, 1.0, 5, 0.8, 0.6, 0.9, 0.3, 0.1, 0.95, 65536, 2, 14, 15, None, 0))
+    assert (e['B'], e['row_len'], e['guided'], e['p'], e['s_out'], e['x0_out']) == (2, 65536, False, 0.95, True, False)
+
+
+def test_entry_reads_glue_and_eft_calls_by_parameter_name():
+    # up, target, H, W, mode, weight, lambda_color, lambda_sil, lambda_opacity, g_extra, sums, g_up, h, w, g_img, g_sil, stream
+    e = sp.entry(_call('sfb_fusion_loss_ex', 1, 2, 128, 96, 1, 0.25, 1.0, 0.5, 0.125, None, 11, 12, 64, 48, 15, 16, 0))
+    assert e == dict(h=64, w=48, mode=1, g_extra=False, wgt=0.25, lam=(1.0, 0.5, 0.125), op='fusion_loss', family='Distill', label='recorded')
+    # x, ldx, y, ldo, NB, H, W, C, Ho, Wo, stream
+    e = sp.entry(_call('sfb_resize_bilinear_ac_nhwc', 1, 12, 3, 20, 2, 5, 7, 8, 16, 9, 0, family='EFT'))
+    assert e == dict(NB=2, H=5, W=7, C=8, Ho=16, Wo=9, ldx=12, ldo=20, op='resize', family='EFT', label='recorded')
+    # x, ldx, grid, out, ldo, NB, H, W, C, M, stream
+    e = sp.entry(_call('sfb_grid_sample_nhwc', 1, 64, 3, 4, 70, 1, 6, 5, 60, 33, 0, family='EFT'))
+    assert e == dict(NB=1, H=6, W=5, C=60, M=33, ldx=64, ldo=70, op='grid_sample', family='EFT', label='recorded')
+    assert sp.entry(_call('sfb_relu_nhwc', 1, 64, 0)) is None
+    assert sp.entry(insitu.Rec('groupnorm', {}, (), {})) is None
