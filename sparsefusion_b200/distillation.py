@@ -697,7 +697,10 @@ class Distiller:
                     start_percep_step=self.start_percep_step, plms_steps=self.sampler.plms_steps, fused_glue=self.fused_glue,
                     percep=self.percep is not None, z_scale_factor=self.z_scale_factor, keyed=self._keyed,
                     # only when on: checkpoints made before the entropy term existed carry no such key and continue at lambda_entropy 0
-                    **({'lambda_entropy': self.lambda_entropy} if self.lambda_entropy != 0 else {}))
+                    **({'lambda_entropy': self.lambda_entropy} if self.lambda_entropy != 0 else {}),
+                    # likewise for pretrained perceptual weights (``percep_weights``): a run with them and one with the random initialisation
+                    # distil different losses
+                    **({'percep_pretrained': True} if getattr(self.percep, 'pretrained', False) else {}))
 
     def _scene_state(self, itr, use_diffusion):
         """this scene's part of a checkpoint: everything but the global generators"""
@@ -1132,7 +1135,8 @@ class NativeSceneBuilder:
 def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx,
                       use_diffusion=True, max_itr=3000, loss_fn_vgg=None, *, scene_builder=None, views_per_step=None, on_iteration=None, seed=None,
                       process_group=None, evaluate=False, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                      cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None):
+                      cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None,
+                      percep_weights=None):
     """sparsefusion/distillation.py:26-497 with the reference's signature (demo.py:87-103 calls it unchanged): builds the per-scene cache
     (``ReferenceSceneBuilder``, or ``scene_builder.build(...)``), optimises a fresh ``NeRFNetwork(opt)`` for ``max_itr`` iterations with
     ``Distiller.step`` and saves ``{'model_state_dict': ngp.state_dict()}`` to ``{save_dir}/{seq_name}.pt`` (:495-496).
@@ -1195,6 +1199,11 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ``Distiller.check_state``) is a ValueError.  With ``max_itr`` at or below the saved iteration no iteration runs and the outputs come from
     the saved state, so a finished run with a checkpoint can be extended by a larger ``max_itr``; without a checkpoint the run starts fresh,
     so an interrupted command can be re-issued unchanged.
+
+    ``percep_weights`` (a state dict in ``lpips.LPIPS(net='vgg')``'s key layout, e.g. ``loss_fn_vgg.state_dict()`` or
+    ``lpips_vgg.load_lpips_state_dict(path)``) is loaded into the loop's ``PerceptualLoss`` before the first iteration, so the perceptual
+    term of the fusion loss is the reference's pretrained LPIPS-VGG (:161, :312-314).  None (the default) keeps ``PerceptualLoss``'s seeded
+    random initialisation.  The checkpoint fingerprint records pretrained weights, so a resume that mixes the two is a ValueError.
     Returns the optimised network."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distillation_loop')
@@ -1213,14 +1222,15 @@ def distillation_loop(gpu, args, opt, model_tuple, save_dir, seq_name, scene_cam
     ngp_network, = _run_distillation(gpu, args, opt, eft, save_dir, [(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)],
                                      make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate, loss_fn_vgg, visualize,
                                      visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale), checkpoint_every, resume,
-                                     progress_every)
+                                     progress_every, percep_weights)
     print('input idx', input_idx)
     return ngp_network
 
 
 def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusion=True, max_itr=3000, scene_builder=None, seed=None, on_iteration=None,
                    evaluate=False, loss_fn_vgg=None, visualize=False, visualize_shadings=(), evaluate_baselines=False, vldm_cond_scale=1.0,
-                   cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None):
+                   cond_scale=1.0, sds_method='plms', checkpoint_every=None, resume=False, lambda_entropy=0.0, progress_every=None,
+                   percep_weights=None, seeds=None):
     """``distillation_loop`` for several scenes at once on one GPU (``MultiSceneDistiller``): demo.py's per-scene loop (demo.py:87-103) becomes
     one call.  ``scenes`` is a list of ``(seq_name, scene_cameras, scene_rgb, scene_mask, scene_valid_region, input_idx)``, the per-scene
     arguments demo.py passes to ``distillation_loop``.  Each scene's cache is built as ``distillation_loop`` builds it (``ReferenceSceneBuilder``,
@@ -1238,21 +1248,35 @@ def distill_scenes(gpu, args, opt, model_tuple, save_dir, scenes, *, use_diffusi
     of ``MultiSceneDistiller.state_dict``).  Resuming needs a checkpoint at the same iteration for every scene of the call, or none (then
     the call starts fresh); anything else is a ValueError naming the scenes.  ``lambda_entropy`` / ``progress_every``: as
     ``distillation_loop``'s, every scene's entropy weight, history and progress files, scene k's snapshot jitter keyed by ``seed + k``.
+    ``percep_weights``: as ``distillation_loop``'s, loaded into the one ``PerceptualLoss`` of all scenes.
+
+    ``seeds`` (one non-negative int per scene, instead of ``seed``) seeds scene k with ``seeds[k]`` wherever the above says ``seed + k``, and
+    also seeds torch's global CPU generator with ``seeds[k]`` immediately before scene k's cache is built; that stream serves the scene's
+    circle-path jitter (``NativeSceneBuilder``) and then its network's initialisation.  A scene's outputs then depend on its own seed and
+    inputs only, not on which other scenes share the call or their order.  Its checkpoint stores ``seeds[k]`` (and no base seed); resuming
+    it under another seed, or with ``seed`` instead of ``seeds``, or the other way round, is a ValueError.
     Returns the optimised networks in the order of ``scenes``."""
     eft, vae, vldm = model_tuple
     _check_sds_method(sds_method, 'distill_scenes')
     _check_lambda_entropy(lambda_entropy, 'distill_scenes')
     if use_diffusion:
         _check_cond_scale(vldm, cond_scale, 'distill_scenes')
+    if seeds is not None:
+        if seed is not None:
+            raise ValueError('distill_scenes: pass seed (scene k seeded seed + k) or seeds (one per scene), not both')
+        seeds = list(seeds)
+        if len(seeds) != len(scenes) or not all(isinstance(s, int) and not isinstance(s, bool) and 0 <= s < 2 ** 63 for s in seeds):
+            raise ValueError(f'distill_scenes: seeds must hold one int in [0, 2**63) per scene ({len(scenes)} scenes, got {seeds!r})')
 
-    def make(ngps, caches, percep, base):
-        return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=[base + k for k in range(len(ngps))], percep=percep,
+    def make(ngps, caches, percep, base):       # base: the base seed, or the list of per-scene seeds
+        scene_seeds = list(base) if isinstance(base, list) else [base + k for k in range(len(ngps))]
+        return MultiSceneDistiller(ngps, vae, vldm, opt, caches, seeds=scene_seeds, percep=percep,
                                    plms_steps=50, start_fusion_step=1000, lambda_color=1.0, lambda_sil=1.0, lambda_opacity=1e-3,   # :148-160
                                    lambda_percep=0.1, start_percep_step=1000, cond_scale=cond_scale if use_diffusion else 1.0, sds_method=sds_method,
                                    lambda_entropy=lambda_entropy, max_itr=max_itr)
     return _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate,
                              loss_fn_vgg, visualize, visualize_shadings, _baselines(evaluate_baselines, vae, vldm, vldm_cond_scale),
-                             checkpoint_every, resume, progress_every)
+                             checkpoint_every, resume, progress_every, percep_weights, seeds)
 
 
 def _baselines(enabled, vae, vldm, cond_scale):
@@ -1333,9 +1357,10 @@ def _checkpoint_paths(save_dir, scenes):
     return [f'{save_dir}/checkpoints/{sc[0]}.ckpt' for sc in scenes]
 
 
-def _read_checkpoints(paths, names, seed):
+def _read_checkpoints(paths, names, seed, seeds=None):
     """the scenes' saved states for ``resume``, or None when no scene has one; ValueError when only some have one, when they are at
-    different iterations or base seeds, or when an explicit ``seed`` differs from the saved base seed"""
+    different iterations or base seeds, or when an explicit ``seed`` differs from the saved base seed.  With per-scene ``seeds``
+    (``distill_scenes``): ValueError unless every scene was saved with its own seed (base seed None) equal to ``seeds[k]``."""
     have = [os.path.exists(p) for p in paths]
     if not any(have):
         return None
@@ -1346,6 +1371,17 @@ def _read_checkpoints(paths, names, seed):
     itrs = {n: s['itr'] for n, s in zip(names, states)}
     if len(set(itrs.values())) > 1:
         raise ValueError(f'resume: the scenes\' checkpoints are at different iterations {itrs}; a call resumes scenes saved together')
+    if seeds is not None:
+        for n, s, want in zip(names, states, seeds):
+            if s['base_seed'] is not None:
+                raise ValueError(f'resume: scene {n} was saved by a run with seed={s["base_seed"]} (scene k seeded seed + k); this call passes '
+                                 f'seeds')
+            if s['seed'] != want:
+                raise ValueError(f'resume: scene {n} was saved with seed {s["seed"]}, this call passes {want} in seeds')
+        return states
+    unseeded = [n for n, s in zip(names, states) if s['base_seed'] is None]
+    if unseeded:
+        raise ValueError(f'resume: scenes {unseeded} were saved by a run with per-scene seeds; resume them with the same seeds')
     bases = {n: s['base_seed'] for n, s in zip(names, states)}
     if len(set(bases.values())) > 1:
         raise ValueError(f'resume: the scenes\' checkpoints come from different runs (base seeds {bases})')
@@ -1356,8 +1392,9 @@ def _read_checkpoints(paths, names, seed):
 
 
 def _write_checkpoints(dist, paths, itr, use_diffusion, base_seed):
-    """every scene's checkpoint at iteration ``itr`` (the next one to run); with a process group every rank takes part in gathering the
-    generator states, rank 0 writes and all ranks wait at a barrier"""
+    """every scene's checkpoint at iteration ``itr`` (the next one to run), each with the call's ``base_seed`` (None for a call with
+    per-scene seeds; every scene's state holds its own seed); with a process group every rank takes part in gathering the generator
+    states, rank 0 writes and all ranks wait at a barrier"""
     sd = dist.state_dict(itr, use_diffusion)
     states = sd['scenes'] if isinstance(dist, MultiSceneDistiller) else [sd]
     pg = getattr(dist, 'pg', None)
@@ -1371,20 +1408,21 @@ def _write_checkpoints(dist, paths, itr, use_diffusion, base_seed):
 
 def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion, max_itr, scene_builder, seed, on_iteration, evaluate=False,
                       loss_fn_vgg=None, visualize=False, visualize_shadings=(), baselines=None, checkpoint_every=None, resume=False,
-                      progress_every=None):
+                      progress_every=None, percep_weights=None, seeds=None):
     """what ``distillation_loop`` and ``distill_scenes`` share: the reference's output directories, one cache per scene of ``scenes`` (as
-    ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds, the
-    ``max_itr`` iterations and one saved network per scene; with ``evaluate``, the scene scores and metrics files, with ``visualize`` the EFT
-    grids before the loop and the gifs and jpegs after it (scene k seeded ``seed + k``); with ``baselines`` (``_baselines``), the EFT and VLDM
-    scores, metrics files and gifs after it; with ``checkpoint_every`` / ``resume`` the checkpoints and with ``progress_every`` the progress
-    files of ``distillation_loop``'s docstring.  Returns the networks."""
+    ``distill_scenes`` takes them), a fresh ``NeRFNetwork(opt)`` per scene, the distiller ``make(ngps, caches, percep, seed)`` builds
+    (``seed``: the base seed, or the list ``seeds``), the ``max_itr`` iterations and one saved network per scene; with ``evaluate``, the scene scores and metrics files, with
+    ``visualize`` the EFT grids before the loop and the gifs and jpegs after it (scene k seeded ``scene_seeds[k]``: ``seed + k``, or
+    ``seeds[k]``, which also seeds the global CPU generator before the scene's cache and network); with ``baselines`` (``_baselines``), the
+    EFT and VLDM scores, metrics files and gifs after it; with ``checkpoint_every`` / ``resume`` the checkpoints, with ``progress_every`` the
+    progress files and with ``percep_weights`` the pretrained perceptual term of ``distillation_loop``'s docstring.  Returns the networks."""
     from .lpips_vgg import PerceptualLoss
     from .progress import ProgressWriter, check_progress_every
     check_progress_every(progress_every)
     if checkpoint_every is not None and (isinstance(checkpoint_every, bool) or not isinstance(checkpoint_every, int) or checkpoint_every < 1):
         raise ValueError(f'checkpoint_every must be a positive int or None (got {checkpoint_every!r})')
     ckpt_paths = _checkpoint_paths(save_dir, scenes)
-    saved = _read_checkpoints(ckpt_paths, [sc[0] for sc in scenes], seed) if resume else None
+    saved = _read_checkpoints(ckpt_paths, [sc[0] for sc in scenes], seed, seeds) if resume else None
     builder = scene_builder if scene_builder is not None else ReferenceSceneBuilder(gpu)
     visualize_shadings = tuple(visualize_shadings)
     if not all(isinstance(sh, str) and sh and '/' not in sh for sh in visualize_shadings):
@@ -1415,8 +1453,12 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
     input_views = [_view_rows(v, sc[5]).to(device) for v, sc in zip(all_views, scenes)] if progress_every is not None else None
     del all_views
     circles = [tuple(t.to(device) for t in builder.circle_views(cams)) for _, cams, _, _, _, _ in scenes] if visualize else None
-    caches = [builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device)
-              for _, cams, rgb, mask, _, input_idx in scenes]
+    caches, cpu_streams = [], []
+    for k, (_, cams, rgb, mask, _, input_idx) in enumerate(scenes):
+        if seeds is not None:
+            torch.default_generator.manual_seed(seeds[k])
+        caches.append(builder.build(eft, cams, rgb, mask, input_idx, use_diffusion=use_diffusion).to(device))
+        cpu_streams.append(torch.get_rng_state())      # where scene k's network initialisation continues its stream (with seeds)
     if baselines is not None:
         from .baselines import check_baseline_cache
         for views, cache in zip(eval_views, caches):
@@ -1432,12 +1474,22 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
                 _write_eft_grid(f'{exp_dir}/log/{seq_name}_eft_grid.jpg', cache.target_eft_image, views.rgb.shape[0])   # :129-141
     with torch.cuda.device(device):
         perceptual_loss = PerceptualLoss('vgg', device=device) if use_diffusion else None                          # :161
-        ngps = [NeRFNetwork(opt).to(device).train() for _ in scenes]                                               # :164
-        if saved is not None:
-            base_seed = saved[0]['base_seed']
+        if perceptual_loss is not None and percep_weights is not None:
+            perceptual_loss.load_state_dict(percep_weights)
+        ngps = []
+        for k in range(len(scenes)):
+            if seeds is not None:
+                torch.set_rng_state(cpu_streams[k])
+            ngps.append(NeRFNetwork(opt).to(device).train())                                                       # :164
+        if seeds is not None:
+            base_seed, scene_seeds = None, list(seeds)
         else:
-            base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
-        dist = make(ngps, caches, perceptual_loss, base_seed)
+            if saved is not None:
+                base_seed = saved[0]['base_seed']
+            else:
+                base_seed = torch.seed() % (2 ** 31) if seed is None else int(seed)
+            scene_seeds = [base_seed + k for k in range(len(scenes))]
+        dist = make(ngps, caches, perceptual_loss, scene_seeds if seeds is not None else base_seed)
         progress = None
         if progress_every is not None and getattr(dist, 'rank', 0) == 0:
             progress = ProgressWriter(exp_dir, [sc[0] for sc in scenes], input_views, [sc[5] for sc in scenes], opt)
@@ -1467,18 +1519,18 @@ def _run_distillation(gpu, args, opt, eft, save_dir, scenes, make, use_diffusion
             for k, ((seq_name, *_rest), ngp, views) in enumerate(zip(scenes, ngps, eval_views)):
                 scores = None
                 if evaluate:
-                    scores = evaluate_scene(ngp, views, opt, eval_percep, seed=base_seed + k)                       # :391-433
+                    scores = evaluate_scene(ngp, views, opt, eval_percep, seed=scene_seeds[k])                    # :391-433
                     print('warning: this metric is used for debugging only and not the final metric')
                     print(f'{getattr(args, "category", "")} scene {seq_name}')
                     write_scene_metrics(f'{save_dir}/metrics/{seq_name}.txt', scores)                              # :434-441
                 if visualize:
                     _write_scene_pictures(save_dir, seq_name, ngp, opt, views, circles[k], caches[k].target_eft_image if use_diffusion else None,
-                                          base_seed + k, scores, visualize_shadings)                                # :444-493
+                                          scene_seeds[k], scores, visualize_shadings)                                 # :444-493
             if baselines is not None:
                 from .baselines import evaluate_baselines
                 sampler = PLMSSampler(baselines['vldm'], 50)                                                        # plms_steps of the loop (:160)
                 for k, ((seq_name, *_rest), views) in enumerate(zip(scenes, eval_views)):
-                    evaluate_baselines(save_dir, seq_name, baselines['vldm'], baselines['vae'], caches[k], views, eval_percep, seed=base_seed + k,
+                    evaluate_baselines(save_dir, seq_name, baselines['vldm'], baselines['vae'], caches[k], views, eval_percep, seed=scene_seeds[k],
                                        cond_scale=baselines['cond_scale'], sampler=sampler)
     return ngps
 

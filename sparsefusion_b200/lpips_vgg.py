@@ -7,7 +7,8 @@ Same call: ``PerceptualLoss('vgg', device)(pred, target, normalize=True) -> [B,1
 no_grad, distillation.py:302-309).
 
 ``state_dict`` keys follow the ``lpips`` package (``net.slice{1..5}.{torchvision index}.weight/bias``, ``lin{k}.model.1.weight``), so the package's
-weights load unchanged; this repository cannot ship them (no network), so a fresh module is randomly initialised and says so.
+weights load unchanged; this repository cannot ship them, so a fresh module is randomly initialised and says so (``pretrained``).
+``load_lpips_state_dict`` reads the pretrained weights from a local file or from the two files the ``lpips`` package is built from.
 
 Engine (CUDA only, C ABI section 7): both images go through the VGG16 trunk as ONE batch of two NHWC tensors; the 13 convolutions and, for the
 gradient, their 13 data-gradient convolutions (same kernel, weights transposed and flipped) run on the wgmma 3xTF32 implicit-GEMM engine with
@@ -33,6 +34,42 @@ CHNS = (64, 128, 256, 512, 512)
 
 def conv_names() -> List[str]:
     return [f'net.slice{s}.{i}' for s, i in zip(SLICE_OF, TV_INDEX)]
+
+
+LPIPS_LIN_FILE = 'vgg.pth'                    # the lpips package's weights/v0.1/vgg.pth: the lin{k}.model.1.weight heads
+TORCHVISION_VGG16_FILE = 'vgg16-397923af.pth'  # torchvision's ImageNet VGG-16: features.{N}.weight / .bias
+
+
+def _lpips_keys() -> List[str]:
+    return [n + s for n in conv_names() for s in ('.weight', '.bias')] + [f'lin{k}.model.1.weight' for k in range(len(CHNS))]
+
+
+def load_lpips_state_dict(path: str) -> Dict[str, torch.Tensor]:
+    """the pretrained LPIPS-VGG weights as a state dict in ``PerceptualLoss``'s (= ``lpips.LPIPS(net='vgg')``'s) key layout, from either
+
+    * a file holding such a state dict, e.g. ``torch.save(lpips.LPIPS(net='vgg').state_dict(), path)`` on a machine with the ``lpips``
+      package (extra keys such as ``scaling_layer.*`` are dropped), or
+    * a directory holding the two files that package builds the network from: its ``weights/v0.1/vgg.pth`` (``LPIPS_LIN_FILE``, the
+      ``lin*`` heads) and torchvision's ``vgg16-397923af.pth`` (``TORCHVISION_VGG16_FILE``, whose ``features.N`` convolutions become
+      ``net.sliceK.N``).
+
+    Files are read with ``torch.load(weights_only=True)``.  RuntimeError naming the keys when any LPIPS key is missing."""
+    import os
+    if os.path.isdir(path):
+        lin = torch.load(os.path.join(path, LPIPS_LIN_FILE), map_location='cpu', weights_only=True)
+        vgg = torch.load(os.path.join(path, TORCHVISION_VGG16_FILE), map_location='cpu', weights_only=True)
+        src = {f'lin{k}.model.1.weight': lin[f'lin{k}.model.1.weight'] for k in range(len(CHNS)) if f'lin{k}.model.1.weight' in lin}
+        for name, i in zip(conv_names(), TV_INDEX):
+            for s in ('weight', 'bias'):
+                if f'features.{i}.{s}' in vgg:
+                    src[f'{name}.{s}'] = vgg[f'features.{i}.{s}']
+    else:
+        src = torch.load(path, map_location='cpu', weights_only=True)
+    keys = _lpips_keys()
+    missing = [k for k in keys if k not in src]
+    if missing:
+        raise RuntimeError(f'load_lpips_state_dict({path!r}): {len(missing)} LPIPS-VGG weights missing, e.g. {missing[:4]}')
+    return {k: src[k] for k in keys}
 
 
 class PerceptualLoss(nn.Module):

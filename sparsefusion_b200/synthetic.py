@@ -55,3 +55,47 @@ def synthetic_scene(n_input=2, n_target=64, image_size=256, latent=32, feat_ch=2
         target_features=torch.from_numpy(rng.standard_normal((n_target, feat_ch, latent, latent), dtype=np.float32)),
         target_eft_image=torch.from_numpy(rng.random((n_target, 3, image_size, image_size), dtype=np.float32) * disc),
         target_rays_o=tro, target_rays_d=trd)
+
+
+def toy_scene(k: int, n_views: int = 12) -> dict:
+    """scene k of a synthetic toy dataset in the reference's layout (utils/co3d_toy_dataloader.py): ``n_views`` pytorch3d cameras on a
+    ``circle_cameras`` ring (radius and elevation vary with k) looking at a lit disc, R [N,3,3], T [N,3], f [N,2], c [N,2], image_size,
+    images [N,3,256,256], masks and valid_region [N,1,256,256]"""
+    g = torch.Generator().manual_seed(100 + k)
+    R, T = [], []
+    for c, rows in circle_cameras(n_views, radius=4.0 + 0.5 * k, elevation_deg=10.0 + 5 * k):
+        r = torch.from_numpy(rows).T.contiguous()          # x_view = x_world R + T: R's columns are the camera axes
+        R.append(r)
+        T.append(-torch.from_numpy(c) @ r)
+    yy, xx = torch.meshgrid(torch.arange(256.0), torch.arange(256.0), indexing='ij')
+    disc = (((yy - 128) ** 2 + (xx - 128) ** 2) < (70 + 5 * k) ** 2).float()
+    images = (torch.rand(n_views, 3, 1, 1, generator=g) * 0.8 + 0.2) * disc
+    return dict(R=torch.stack(R), T=torch.stack(T), f=torch.full((n_views, 2), 3.0), c=torch.zeros(n_views, 2),
+                image_size=torch.full((n_views, 2), 256.0), images=images, masks=disc.expand(n_views, 1, 256, 256).clone(),
+                valid_region=torch.ones(n_views, 1, 256, 256))
+
+
+def write_demo_inputs(d: str, cat: str = 'hydrant', n_scenes: int = 2, n_views: int = 12, seed: int = 0) -> dict:
+    """what ``python -m sparsefusion_b200.demo`` reads, with random weights: ``{d}/data/{cat}/{cat}_toy.pt`` (``toy_scene`` 0..n_scenes-1),
+    the EFT, VLDM and SD-VAE checkpoints of the released configuration in the released files' layouts, and LPIPS-VGG weights.  Returns
+    the paths (root, eft, vldm, vae, lpips) and the LPIPS state dict (lpips_sd)."""
+    import os
+    from . import demo
+    from .eft import EpipolarFeatureTransformer
+    from .imagen_pytorch import Unet
+    from .ldm_autoencoder import AutoencoderKL
+    from .lpips_vgg import PerceptualLoss
+    from .vldm import DDPM
+    os.makedirs(f'{d}/data/{cat}', exist_ok=True)
+    torch.save({cat: [toy_scene(k, n_views) for k in range(n_scenes)]}, f'{d}/data/{cat}/{cat}_toy.pt')
+    torch.manual_seed(seed)
+    eft = EpipolarFeatureTransformer(use_r=True, encoder='resnet18', return_features=True, remove_unused_layers=False)
+    torch.save({'model_state_dict': eft.state_dict()}, f'{d}/eft.pt')
+    vldm = DDPM(unets=(Unet(**demo.UNET_KW),), **demo.DDPM_KW)
+    torch.save({'model_state_dict': vldm.state_dict()}, f'{d}/vldm.pt')
+    del vldm
+    vae = AutoencoderKL(**demo.VAE_KW)
+    torch.save({'state_dict': {f'first_stage_model.{k}': v for k, v in vae.state_dict().items()}}, f'{d}/vae.ckpt')
+    lp = PerceptualLoss('vgg', seed=seed + 11).state_dict()
+    torch.save(lp, f'{d}/lpips.pt')
+    return dict(root=f'{d}/data', eft=f'{d}/eft.pt', vldm=f'{d}/vldm.pt', vae=f'{d}/vae.ckpt', lpips=f'{d}/lpips.pt', lpips_sd=lp)
